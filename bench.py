@@ -36,6 +36,7 @@ ALG_K1A = 66.2                        # 2 PCM + 16 AGC ring + 32 EbNo rings + 16
 ALG_K2 = 128.0                        # estimator frame traffic: 32*nfft bytes per nfft/4 samples
 ALG_STEP = 194.2                      # the whole step (K1a + K2)
 ALG_MSK = 2 + 16 + 32 + 16 + 128 + 0.05   # same accounting for the MSK path (nfft 8192 per 2048 samples -> 128 B/sample)
+HBM_GBS_DATASHEET = 3350.0            # H100 SXM HBM3, NVIDIA data sheet: the roofline denominator when MEASURED_PEAKS.json is absent
 
 MODES = {
     "oqpsk10500": dict(kind="oqpsk", fb=10500, fc0=8000, fc_span=500, lockingbw=10500, ebn0=10.0, channels=4096, frames=2,
@@ -63,7 +64,14 @@ def parse():
     ap.add_argument("--streams", type=int, default=1, help="continuous workloads: split a GPU's channels into this many batches, each on its own CUDA stream "
                     "(the demodulator epoch of one batch then overlaps the estimator epoch of another)")
     ap.add_argument("--scaling", default="weak", choices=["weak", "strong"], help="mix16384: weak = 2048 channels per GPU, strong = 16384 in total")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="continuous workloads: after the timed steps write what the last timed step returned (rank 0's channels) as DIR/<name>.npy")
+    a = ap.parse_args()
+    if a.steps < 1:
+        ap.error("--steps must be at least 1")
+    if a.dump_outputs and (a.workload not in MODES or a.impl != "ours"):
+        ap.error("--dump-outputs is implemented for the continuous workloads of the CUDA path (%s)" % ", ".join(MODES))
+    return a
 
 
 # ----------------------------------------------------------------------------- synthetic input
@@ -274,23 +282,6 @@ def load_peaks():
         return {}
 
 
-def ncu_traffic_bytes(kernel):
-    """dram__bytes_read.sum + dram__bytes_write.sum of one launch of `kernel`, from this round's committed `ncu --set full`
-    capture profiles/r02_<kernel>_full_raw.csv (None if that capture is absent: never a stale round's number)."""
-    import csv
-    path = os.path.join(ROOT, "profiles", "r02_%s_full_raw.csv" % kernel)
-    try:
-        rows = list(csv.reader(open(path)))
-        hdr, units, row = rows[0], rows[1], rows[2]
-        tot = 0.0
-        for k in ("dram__bytes_read.sum", "dram__bytes_write.sum"):
-            i = hdr.index(k)
-            tot += float(row[i].replace(",", "")) * {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}[units[i]]
-        return tot, os.path.relpath(path, ROOT)
-    except Exception:
-        return None, None
-
-
 class Pipeline:
     """One continuous-mode batch + its frame layer on one GPU, with the PCM of one step resident in HBM."""
 
@@ -306,11 +297,12 @@ class Pipeline:
         self.stream = stream
         self.stride = self.pcm.stride(0)
 
-    def step_device(self):
+    def step_device(self, keep_sus=False):
         self.batch.write_device(self.pcm.data_ptr(), STEP_SAMPLES, self.stride)
         self.layer.process_batch(self.batch)
         self.layer.tick(self.batch)
-        self.layer.discard_sus()          # results stay on the device for the HBM-resident measurement
+        if not keep_sus:
+            self.layer.discard_sus()      # results stay on the device for the HBM-resident measurement
 
     @property
     def launches(self):
@@ -320,8 +312,9 @@ class Pipeline:
         self.batch.close(); self.layer.close()
 
 
-def timed_steps(pipes, stream, steps, warmup, rank, local, dev):
-    """W warm-up steps, then exactly K steps between CUDA events on the launching stream; max over ranks."""
+def timed_steps(pipes, stream, steps, warmup, rank, local, dev, keep_last=False):
+    """W warm-up steps, then exactly K steps between CUDA events on the launching stream; max over ranks.
+    keep_last: the last step leaves its signal units queued for dump_outputs instead of discarding them."""
     import torch
     from jaero_b200 import shard
     clocks = ClockSampler(local)
@@ -341,9 +334,9 @@ def timed_steps(pipes, stream, steps, warmup, rank, local, dev):
     e0.record(stream)
     for so in others:
         so.wait_event(e0)                 # no batch starts before e0 ...
-    for _ in range(steps):
+    for k in range(steps):
         for p in pipes:
-            p.step_device()
+            p.step_device(keep_sus=keep_last and k == steps - 1)
     for so in others:
         ej = torch.cuda.Event(); ej.record(so); stream.wait_event(ej)   # ... and e1 fires when every batch is done
     e1.record(stream)
@@ -358,22 +351,52 @@ def timed_steps(pipes, stream, steps, warmup, rank, local, dev):
     return ms, ms_local, launches, profs, clk
 
 
-def roofline_block(mode, prof, C, ms_local, peaks):
+DUMP_LIMIT = 64 << 20                 # bytes: larger outputs are dumped for a fixed, seeded sample of channels
+
+
+def dump_outputs(pipes, out_dir):
+    """What a caller of the timed path receives after its last step, channels in order across the batches: the signal-unit
+    records (12 SU bytes, CRC flag, index in frame, frame number lo/hi) and their counts, the P-channel statistics and the
+    demodulator status. Written as float32 / float64 .npy files."""
+    recs, counts, stats, status = [], [], [], []
+    for p in pipes:
+        r, c = p.layer.read_sus_raw(out=np.zeros((p.C, p.layer.su_cap, 16), dtype=np.uint8))   # zero past each channel's count
+        recs.append(r); counts.append(c)
+        stats.append(np.stack(p.layer.stats(), axis=1))
+        st = p.batch.status()
+        status.append(np.array([[s[f] for f in STATUS_FIELDS] for s in st], dtype=np.float64))
+    out = {"su_records": np.concatenate(recs).astype(np.float32), "su_counts": np.concatenate(counts).astype(np.float32),
+           "pchannel_stats": np.concatenate(stats).astype(np.float64), "demod_status": np.concatenate(status)}
+    C = len(out["su_counts"])
+    per_channel = sum(v.nbytes for v in out.values()) / C
+    if per_channel * C > DUMP_LIMIT:
+        keep = np.sort(np.random.default_rng(0).choice(C, int(DUMP_LIMIT // per_channel), replace=False))
+        out = {k: v[keep] for k, v in out.items()}
+        out["channel_index"] = keep.astype(np.float64)
+    os.makedirs(out_dir, exist_ok=True)
+    for k, v in out.items():
+        np.save(os.path.join(out_dir, k + ".npy"), v)
+    return sorted(out)
+
+
+STATUS_FIELDS = ("mixer2_freq", "mixer2_wtptr", "center_freq", "st_freq", "st_wtptr", "agc", "mse", "ebno", "marg", "cfe_est",
+                 "n_sig_true", "n_sig_false", "samples", "softbits", "dcd", "peak_volume")
+
+
+def roofline_block(mode, prof, C, ms_local, peaks, cfe_clusters):
     m = MODES[mode]
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", HBM_GBS_DATASHEET))
     seg_s, cfe_s = prof["segment_ms"] * 1e-3, prof["cfe_ms"] * 1e-3
     units = prof["samples"] * C                                   # channel-samples the timed launches processed
     ach = (m["alg"] * units) / seg_s / 1e9 if seg_s > 0 else 0.0
     ach2 = (ALG_K2 * units) / cfe_s / 1e9 if cfe_s > 0 else 0.0
     step_ach = ((m["alg"] + ALG_K2) * units) / (ms_local * 1e-3) / 1e9
-    traffic, src = ncu_traffic_bytes(m["kernel"])
     return {"bound": "hbm", "kernel": m["kernel"], "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
-            "traffic": traffic, "traffic_source": src,
-            "peak_source": "measured (MEASURED_PEAKS.json)" if peaks else "fallback (B200_PROFILING.md)",
+            "peak_source": "measured (MEASURED_PEAKS.json)" if peaks else "H100 SXM data sheet (HBM3, 700 W part)",
             "alg_bytes_per_sample": m["alg"], "avg_launch_ms": prof["segment_ms"] / max(1, prof["segment_launches"]),
             "launches": prof["segment_launches"], "share_of_step": prof["segment_ms"] / ms_local,
             "kernels": [
-                {"kernel": "cfe_cluster_kernel+cfe_search_kernel" if mode == "oqpsk10500" else "cfe_col/row kernels", "alg_bytes_per_sample": ALG_K2,
+                {"kernel": "cfe_cluster_kernel+cfe_search_kernel" if cfe_clusters else "cfe_col/row kernels", "cfe_clusters": cfe_clusters, "alg_bytes_per_sample": ALG_K2,
                  "achieved": ach2, "frac": ach2 / peak, "avg_epoch_ms": prof["cfe_ms"] / max(1, prof["cfe_runs"]), "share_of_step": prof["cfe_ms"] / ms_local},
                 {"kernel": "whole step (all kernels)", "alg_bytes_per_sample": m["alg"] + ALG_K2, "achieved": step_ach, "frac": step_ach / peak}],
             "note": "per-channel fp64 feedback loop: bound by dependent-issue latency, not HBM (DESIGN.md section 5); K1a's own algorithmic bytes exclude the estimator's frame traffic, which is K2's"}
@@ -433,7 +456,8 @@ def run_continuous(a, mode):
     pipes = [Pipeline(mode, Cg, ch0 + g * Cg, ebn0, envs_t, dev, local, streams[g]) for g in range(G)]
     pipe = pipes[0]
     torch.cuda.synchronize()
-    ms, ms_local, launches, profs, clk = timed_steps(pipes, stream, a.steps, a.warmup, rank, local, dev)
+    ms, ms_local, launches, profs, clk = timed_steps(pipes, stream, a.steps, a.warmup, rank, local, dev, keep_last=bool(a.dump_outputs))
+    dumped = dump_outputs(pipes, a.dump_outputs) if a.dump_outputs and rank == 0 else None
     st = [p.layer.stats() for p in pipes]
     dcd, su_tot, su_ok = (np.concatenate([x[i] for x in st]) for i in range(3))
     total_samples = float(C) * STEP_SAMPLES * a.steps * world
@@ -473,7 +497,7 @@ def run_continuous(a, mode):
     prof = {k: sum(pr[k] for pr in profs) for k in profs[0]} if G > 1 else profs[0]
     if G > 1:
         prof["samples"] = profs[0]["samples"]; prof["batches"] = G
-    roofline = roofline_block(mode, prof, C, ms_local, peaks)
+    roofline = roofline_block(mode, prof, C, ms_local, peaks, pipes[0].batch.cfe_clusters)
 
     # ---- saturation: what the same pipeline reaches with more channels per GPU (the metric's 4096 leave most issue slots idle)
     saturation = None
@@ -482,7 +506,7 @@ def run_continuous(a, mode):
         pcm0, fcs0 = pipe.pcm, pipe.fcs
         for p in pipes:
             p.close()
-        for Cs in (8192, 16384, 32768):
+        for Cs in (8192, 16384):                  # ~3.4 MB of state per channel: 16384 channels fill ~56 GB of the 80 GB
             try:
                 ps = Pipeline(mode, Cs, 0, ebn0, envs_t, dev, local, stream)
                 for _ in range(2):
@@ -490,14 +514,14 @@ def run_continuous(a, mode):
                 torch.cuda.synchronize()
                 s0, s1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                 s0.record(stream)
-                for _ in range(3):
+                for _ in range(a.steps):
                     ps.step_device()
                 s1.record(stream)
                 torch.cuda.synchronize()
-                msx = s0.elapsed_time(s1) / 3
+                msx = s0.elapsed_time(s1) / a.steps
                 v = Cs * STEP_SAMPLES / (msx * 1e-3) / 1e6
                 saturation.append({"channels": Cs, "value": v, "unit": "Msamples/s", "channels_rt": v * 1e6 / FS, "ms_per_step": msx,
-                                   "frac": (ALG_STEP * v * 1e6 / 1e9) / float(peaks.get("hbm_gbs", 6650.0))})
+                                   "frac": (ALG_STEP * v * 1e6 / 1e9) / float(peaks.get("hbm_gbs", HBM_GBS_DATASHEET))})
                 ps.close(); del ps
                 torch.cuda.empty_cache()
             except Exception as ex:                # e.g. out of memory on a smaller part
@@ -520,11 +544,13 @@ def run_continuous(a, mode):
                 "vs_baseline": None, "dtype": "f64", "data": "synthetic", "channels_rt": value * 1e6 / FS,
                 "config": {"workload": m["label"], "channels_per_gpu": C, "seconds_per_step": 1.0, "ebn0_db": ebn0,
                            "parallelism": "channels sharded x%d GPUs x %d concurrent batches per GPU, no data-path collective" % (world, G),
-                           "l2": "inputs (%.0f MB int16 + %.1f GB of ring state per step) exceed the 126 MB L2" % (C * STEP_SAMPLES * 2 / 1e6, C * 3.4e-3)},
+                           "l2": "inputs (%.0f MB int16 + %.1f GB of ring state per step) exceed the 50 MB L2" % (C * STEP_SAMPLES * 2 / 1e6, C * 3.4e-3)},
                 "e2e": e2e, "gpu_launches": int(launches), "clocks": clk, "roofline": roofline, "cpu_baseline": cpu_base,
                 "decode": {"su_total": tot[0], "su_crc_ok": tot[1], "channels_with_dcd": tot[2]}}
         if saturation is not None:
             line["saturation"] = saturation
+        if dumped is not None:
+            line["dumped_outputs"] = {"dir": a.dump_outputs, "arrays": dumped}
         print(json.dumps(line))
     if pipe is not None:
         for p in pipes:

@@ -1,4 +1,4 @@
-/* jaero_b200 — C ABI of the B200-native JAERO demodulator / Viterbi hot path.
+/* jaero_b200 — C ABI of the H100-native JAERO demodulator / Viterbi hot path.
  *
  * Drop-in boundary (SURVEY.md §8b). Every entry point below replaces a piece of the reference's
  * per-instance C++/Qt interface with a *batched* call over many independent channels; a single
@@ -143,6 +143,9 @@ int jaero_batch_set_stream(jaero_batch *b, void *cuda_stream);
  * out[3]=estimator runs, out[4]=samples per channel covered by the segment launches. */
 int jaero_batch_set_profiling(jaero_batch *b, int enabled);
 int jaero_batch_get_profile(jaero_batch *b, double out[5]);
+/* Coarse-estimator path of the batch: the number of co-resident 8-CTA clusters the nfft 2^14 estimator runs on, or 0 when it
+ * runs as the four-step kernels through global memory (nfft 2^13, JAERO_CFE_CLUSTER=0, or no cluster fits the device). */
+int jaero_batch_cfe_clusters(const jaero_batch *b);
 
 /* ---- K=7 r=1/2 soft Viterbi (polys 109,79), one independent decoder per channel ---- */
 int jaero_viterbi_create(int n_channels, int paddinglength, int device_ordinal, jaero_viterbi **out);

@@ -1,4 +1,4 @@
-"""jaero_b200 — B200-native (sm_100a) batched implementation of JAERO's demodulator + Viterbi hot path.
+"""jaero_b200 — H100-native (sm_90a) batched implementation of JAERO's demodulator + Viterbi hot path.
 
 This module is a thin ctypes loader over the C ABI in include/jaero_b200.h (libjaero_b200.so, built
 in-tree by jaero_b200/build.py). There is no CPU fallback: constructing a batch without the CUDA
@@ -49,7 +49,7 @@ EXPORTS = ["jaero_last_error", "jaero_device_count", "jaero_batch_create", "jaer
            "jaero_batch_softbits_device", "jaero_batch_reset_softbits", "jaero_batch_set_dcd",
            "jaero_batch_set_center_freq", "jaero_batch_set_afc", "jaero_batch_set_sql", "jaero_batch_set_cpu_reduce", "jaero_batch_regroup",
            "jaero_burst_set_afc", "jaero_burst_set_sql", "jaero_batch_get_status", "jaero_batch_get_status_all",
-           "jaero_batch_launch_count", "jaero_batch_set_stream", "jaero_batch_set_profiling",
+           "jaero_batch_launch_count", "jaero_batch_set_stream", "jaero_batch_set_profiling", "jaero_batch_cfe_clusters",
            "jaero_batch_get_profile", "jaero_viterbi_create", "jaero_viterbi_destroy",
            "jaero_viterbi_decode_continuous", "jaero_viterbi_decode_continuous_device", "jaero_viterbi_decode_block",
            "jaero_viterbi_reset", "jaero_viterbi_sync", "jaero_viterbi_launch_count",
@@ -96,6 +96,7 @@ def lib():
         L.jaero_batch_set_stream.argtypes = [vp, vp]
         L.jaero_batch_set_profiling.argtypes = [vp, i]
         L.jaero_batch_get_profile.argtypes = [vp, vp]
+        L.jaero_batch_cfe_clusters.argtypes = [vp]
         L.jaero_viterbi_create.argtypes = [i, i, i, ctypes.POINTER(vp)]
         L.jaero_viterbi_destroy.argtypes = [vp]; L.jaero_viterbi_destroy.restype = None
         L.jaero_viterbi_decode_continuous.argtypes = [vp, vp, sz, i, vp, vp]
@@ -264,6 +265,11 @@ class DemodBatch:
         o = np.zeros(5, dtype=np.float64)
         _check(lib().jaero_batch_get_profile(self.h, _p(o)))
         return dict(segment_ms=o[0], segment_launches=int(o[1]), cfe_ms=o[2], cfe_runs=int(o[3]), samples=int(o[4]))
+
+    @property
+    def cfe_clusters(self):
+        """co-resident 8-CTA clusters of the coarse estimator (0: the four-step kernels through global memory)"""
+        return lib().jaero_batch_cfe_clusters(self.h)
 
     @property
     def launches(self):

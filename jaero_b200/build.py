@@ -1,4 +1,4 @@
-"""Build libjaero_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Build libjaero_b200.so in-tree with nvcc for sm_90a (cross-compiles without a GPU)."""
 import os
 import subprocess
 import sys
@@ -7,7 +7,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libjaero_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "-Xcompiler", "-fno-fast-math"]
 # (source, extra flags). The demodulator kernels keep IEEE mul/add separate so that double arithmetic
 # rounds exactly as the CPU reference does (x86-64 has no implicit FMA contraction).

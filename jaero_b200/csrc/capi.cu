@@ -528,8 +528,8 @@ int jaero_batch_create(const jaero_settings *s, int n_channels, const double *fr
         // to re-centre (FreqOffsetEstimateSlot, oqpskdemodulator.cpp:629-677), so in steady state the estimator kernels can run
         // on a second stream while the next segment is demodulated. Conditions: the warp-specialised 10500 bps kernel, the
         // non-cpuReduce schedule, and a segment grid that is fully resident (a waiting CTA must never keep the estimator's
-        // CTAs from being scheduled). OFF unless JAERO_ASYNC_CFE=1: measured on B200 (4096 channels) the estimator's FP64 work,
-        // when it shares SMs with the latency-bound segment warps, slows both kernels by 3-4x (FP64 pipe contention).
+        // CTAs from being scheduled). OFF unless JAERO_ASYNC_CFE=1: the estimator's FP64 work,
+        // when it shares SMs with the latency-bound segment warps, competes with them for the FP64 pipe.
         cudaDeviceProp prop;
         JB_CUDA(cudaGetDeviceProperties(&prop, device));
         const char *e = getenv("JAERO_ASYNC_CFE");
@@ -589,7 +589,7 @@ int jaero_batch_create(const jaero_settings *s, int n_channels, const double *fr
         c.is8400 = (s->fb == 8400);
         std::vector<double2> tw(c.nfft);
         for (int k = 0; k < c.nfft; k++) { const double a = -2.0 * M_PI * (double)k / (double)c.nfft; tw[k] = make_double2(cos(a), sin(a)); }
-        // channels per pass group: the two work buffers of a group (2 x group x nfft x 16 B) (larger groups amortise launch tails; measured best at >= 512 on B200)
+        // channels per pass group: the two work buffers of a group (2 x group x nfft x 16 B) (larger groups amortise launch tails)
         int grp = 1024;
         if (const char *e = getenv("JAERO_CFE_GROUP")) grp = std::max(1, atoi(e));
         c.group = std::min(n_channels, grp);
@@ -735,6 +735,7 @@ int jaero_batch_get_profile(jaero_batch *b, double out[5])
     b->ev_seg.clear(); b->ev_cfe.clear(); b->prof_samples = 0;
     return JAERO_OK;
 }
+int jaero_batch_cfe_clusters(const jaero_batch *b) { return b ? b->cfe.clusters : 0; }
 int jaero_batch_sync(jaero_batch *b)
 {
     if (!b) { set_error("null handle"); return JAERO_E_ARG; }

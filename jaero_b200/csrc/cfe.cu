@@ -6,7 +6,7 @@
 // -> fold search around the expected symbol-rate lines -> freq_offset_est, plus the
 // emptyingcountdown gate (:134-135) and bigchange() (:84-88).
 //
-// B200 mapping: N = n1*n2 (128x128 for 2^14, 128x64 for 2^13) four-step FFT in double precision.
+// Mapping: N = n1*n2 (128x128 for 2^14, 128x64 for 2^13) four-step FFT in double precision.
 // The three transforms are fused into four memory passes by pairing the steps that work on the
 // same row / column of the n1 x n2 matrix:
 //   P1  column FFT (over r) of the linearised ring + twiddle                       ring -> A

@@ -1,4 +1,4 @@
-// jaero_b200 — shared host/device helpers (product code; sm_100a only).
+// jaero_b200 — shared host/device helpers (product code; sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>

@@ -1,5 +1,5 @@
 // Device-side data layout of the continuous demodulators (K1a OQPSK, K1b MSK) and the coarse
-// frequency estimator (K2). Product code, sm_100a only.
+// frequency estimator (K2). Product code, sm_90a only.
 //
 // One GPU thread owns one channel for the serial part of the loop; everything a channel keeps
 // between samples lives in HBM as structure-of-arrays with the CHANNEL index minor

@@ -28,7 +28,7 @@ __device__ __forceinline__ double fmod360(double p)
 }
 
 // ---- shorter transcendental functions for the feedback loop of the pipelined demodulators. The library versions are exact
-// enough but long dependent chains (measured on B200: atan2 440, tanh 298, hypot 155, division 136 cycles per dependent call);
+// enough but long dependent chains (tools/micro/fastlat.cu measures the cycles per dependent call);
 // these keep the same error class (<= 2 ulp, i.e. the same last-bit differences from glibc that the library calls have) with
 // about half the chain length. Zero / non-finite arguments go to the library call, so the special cases are the library's.
 
@@ -186,7 +186,7 @@ __device__ __forceinline__ void push_soft(const DemodParams &p, int ch, int &cou
 }
 
 
-// ---- bulk asynchronous copies (TMA engine, 1-D form) + mbarrier completion, sm_90+/sm_100a PTX
+// ---- bulk asynchronous copies (TMA engine, 1-D form) + mbarrier completion, sm_90 PTX
 __device__ __forceinline__ unsigned smem_u32(const void *p) { return (unsigned)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(unsigned long long *bar, int count)
 { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory"); }

@@ -72,8 +72,7 @@ oqpsk_pipe_kernel(const __grid_constant__ DemodParams p, const SegmentArgs a, co
     double *dv = reinterpret_cast<double *>(pp_smem_raw + PP_SM_BASE + PP_SM_HAND);               // [PP_DV][32]
     double2 *bbst = reinterpret_cast<double2 *>(pp_smem_raw + PP_SM_BASE + PP_SM_HAND + PP_SM_DV); // [8][32]
     // Role ids: F 0, E 1, T 2, K1 3, K2 4, S 5, A 6 = physical warp. (Warps w and w+4 share an SM sub-partition and its FP64
-    // pipe. Other placements were measured on B200 inside one GPU call, 9-warp CTAs with placeholder warps: {F,S,A | E | T | K1,K2},
-    // {F,A | E,S | T | K1,K2}, {F,S | E,A | T | K1,K2}: all 8 % slower per epoch than this one.)
+    // pipe: F with K2, E with S, T with A; K1 has one to itself.)
     const int lane = threadIdx.x & 31;
     const int warp = (int)(threadIdx.x >> 5);
     // Which channel this lane carries. Channels are independent, so the library may seat them as it likes: it regroups them by

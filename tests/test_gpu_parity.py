@@ -1,4 +1,4 @@
-"""GPU parity tests (pytest -m gpu, run on the B200 box): the CUDA path behind the C ABI against the CPU
+"""GPU parity tests (pytest -m gpu, run on an H100): the CUDA path behind the C ABI against the CPU
 oracle on the same inputs. Integer/byte outputs (soft bits after hard decision, Viterbi bits, SU bytes, CRC
 flags) must be bit-exact; floating-point loop state within 1e-6 relative (north_star allows 1e-4)."""
 import hashlib
@@ -604,18 +604,16 @@ def test_rt_channel_known_answer_r_packets(fb):
 
 
 def test_recording_to_acars_end_to_end():
-    """240 s 10.5k recording -> device demodulator -> device P-channel frame layer -> host reassembly == the ACARS records the
-    reference's own demodulator + reassembly code produce (tests/golden/reasm_golden.json, tools/make_reasm_golden.py)."""
+    """12 s of the 10.5k recording -> device demodulator -> device P-channel frame layer -> host reassembly == the signal units
+    and ACARS records the reference's own demodulator + reassembly code produce (tests/golden/reasm_excerpt_10500.json,
+    tools/make_reasm_golden.py --excerpt)."""
     import json
-    import reasm_synth
     jb = _import()
-    path = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "pcm_full", "oqpsk_10500.npy")
-    if not os.path.exists(path):
-        pytest.skip("full-length recording fixture not present (git-ignored; made by tools/make_fixtures.py)")
-    pcm = np.load(path)
-    with open(os.path.join(os.path.dirname(path), "..", "reasm_golden.json")) as fh:
-        want = json.load(fh)["p_recording_10500"]["records"]
-    want_sus = reasm_synth.unpack_stream(np.load(os.path.join(os.path.dirname(path), "..", "reasm_su_streams.npz"))["p_recording_10500"])
+    pcm = load_excerpt("oqpsk_10500")
+    with open(os.path.join(ROOT, "tests", "golden", "reasm_excerpt_10500.json")) as fh:
+        gold = json.load(fh)
+    want, want_sus = gold["records"], [bytes.fromhex(h) for h in gold["sus"]]
+    assert len(want_sus) >= 500 and sum(1 for w in want if w["message"]) >= 5
     kw = dict(fb=10500, freq_center=5760, lockingbw=10500, fft_power=14, signalthreshold=0.65, afc=True)
     b = jb.DemodBatch("oqpsk", 2, **kw)
     pc = jb.PChannelBatch(2, 10500)
@@ -637,7 +635,7 @@ def test_recording_to_acars_end_to_end():
             drain()
     drain()
     for c in range(2):
-        assert sus[c] == [e[1] for e in want_sus]                        # the CRC-valid signal units, byte for byte
+        assert sus[c] == want_sus                                         # the CRC-valid signal units, byte for byte
         got = rs[c].pop_all()
         assert len(got) == len(want)
         for g, w in zip(got, want):

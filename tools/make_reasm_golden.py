@@ -6,7 +6,10 @@ libjaero_ref_reasm.so = JAERO/aerol.cpp:4-487 compiled verbatim) run over
   (3) seeded synthetic SU streams that exercise multi-block ACARS, interleaved sequences, lost SSUs, parity errors,
       R-channel 1/2/3-SU sequences and the garbage cases.
 The SU byte streams themselves are committed (tests/golden/reasm_su_streams.npz) so the tests need neither the
-recordings nor /root/reference. Build container only."""
+recordings nor /root/reference. Build container only.
+
+`--excerpt` writes tests/golden/reasm_excerpt_10500.json instead: the CRC-valid signal units and the ACARS records of the
+committed 12 s excerpt tests/golden/oqpsk_10500_excerpt.npz (same chain as (1)), the end-to-end golden of the GPU tests."""
 import json
 import os
 import sys
@@ -20,9 +23,10 @@ from oracle import ref, restated  # noqa: E402
 import reasm_synth  # noqa: E402  (tests/reasm_synth.py)
 
 
-def recording_sus(name="oqpsk_10500", kind="oqpsk", kw=None):
+def recording_sus(name="oqpsk_10500", kind="oqpsk", kw=None, pcm=None):
     import multiprocessing as mp
-    pcm = np.load(os.path.join(ROOT, "tests", "golden", "pcm_full", name + ".npy"))
+    if pcm is None:
+        pcm = np.load(os.path.join(ROOT, "tests", "golden", "pcm_full", name + ".npy"))
     kw = kw or dict(fb=10500, freq_center=5760, lockingbw=10500, fft_power=14, signalthreshold=0.65, afc=True)
     ctx = mp.get_context("spawn")
     with ctx.Pool(1) as pool:
@@ -74,7 +78,18 @@ def run_stream(stream):
     return rcs, out
 
 
-if __name__ == "__main__":
+def excerpt_golden():
+    pcm = np.load(os.path.join(ROOT, "tests", "golden", "oqpsk_10500_excerpt.npz"))["pcm"]
+    sus = recording_sus(pcm=pcm)
+    rcs, out = run_stream([("su", bytes(x), False) for x in sus])
+    print("excerpt: records", len(out))
+    with open(os.path.join(ROOT, "tests", "golden", "reasm_excerpt_10500.json"), "w") as fh:
+        json.dump(dict(sus=[bytes(x).hex() for x in sus], records=out), fh, indent=0, sort_keys=True)
+
+
+if __name__ == "__main__" and "--excerpt" in sys.argv:
+    excerpt_golden()
+elif __name__ == "__main__":
     streams = {}
     rec = recording_sus()
     streams["p_recording_10500"] = [("su", bytes(x), False) for x in rec]

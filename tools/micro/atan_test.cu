@@ -1,7 +1,7 @@
 #include <cstdio>
 #include <cmath>
 #include <cstdlib>
-#include "/root/repo/jaero_b200/csrc/demod_device.cuh"
+#include "../../jaero_b200/csrc/demod_device.cuh"
 __global__ void k(const double *y, const double *x, double *o, int n) { int i = blockIdx.x*blockDim.x+threadIdx.x; if (i<n) o[i] = jb::atan2_fast(y[i], x[i]); }
 int main(){ const int n=1<<22; double *y,*x,*o; cudaMallocManaged(&y,n*8); cudaMallocManaged(&x,n*8); cudaMallocManaged(&o,n*8);
  srand(1); for(int i=0;i<n;i++){ double a=(rand()/(double)RAND_MAX*2-1), b=(rand()/(double)RAND_MAX*2-1); double s=pow(10.0,(rand()%40)-20); y[i]=a*s; x[i]=b*s*(i%3==0?1e-3:1); }

@@ -1,4 +1,4 @@
-// Micro-benchmark: latency of a warp-to-warp hand-off inside one CTA (B200): named barriers vs shared-memory flags vs mbarriers.
+// Micro-benchmark: latency of a warp-to-warp hand-off inside one CTA: named barriers vs shared-memory flags vs mbarriers.
 #include <cstdio>
 #include <cuda_runtime.h>
 __device__ __forceinline__ void nb_arrive(int id) { asm volatile("bar.arrive %0, 64;" ::"r"(id) : "memory"); }

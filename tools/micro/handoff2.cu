@@ -1,6 +1,6 @@
-// Micro-benchmark (next experiments for the K1a pipeline): does the 87-cycle named-barrier hop depend on WHERE the two warps
+// Micro-benchmark (next experiments for the K1a pipeline): does the named-barrier hop latency depend on WHERE the two warps
 // sit (same SM sub-partition = warp ids equal mod 4, or different ones), and is an mbarrier hand-off any faster?
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o handoff2 handoff2.cu && ./handoff2
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o handoff2 handoff2.cu && ./handoff2
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>

@@ -1,7 +1,7 @@
 #include <cstdio>
 #include <cmath>
 #include <cstdlib>
-#include "/root/repo/jaero_b200/csrc/demod_device.cuh"
+#include "../../jaero_b200/csrc/demod_device.cuh"
 __global__ void k(const double *x, int *o, int n) { int i = blockIdx.x*blockDim.x+threadIdx.x; if (i<n) o[i] = jb::osc_index(x[i]); }
 int main(){ const int n=1<<22; double *x; int *o; cudaMallocManaged(&x,n*8); cudaMallocManaged(&o,n*4);
  srand(3); for(int i=0;i<n;i++){ x[i]=rand()/(double)RAND_MAX*20010.0; if(i%7==0) x[i]=floor(x[i]); if(i%11==0) x[i]=nextafter(floor(x[i]),-1.0); if(i%13==0) x[i]=floor(x[i])+0.5; }
