@@ -66,9 +66,8 @@ __device__ __forceinline__ double atan2_fast(double y, double x)
     return y < 0.0 ? -r : r;
 }
 
-// (Shorter versions of hypot - sqrt(fma(x,x,y*y)) - and tanh - 1 - 2/(exp(2|x|)+1) - were measured too: within 2 ulp of the
-// library, but the kernel got SLOWER with them (divergent branches in tanh, and no gain from hypot), so the library calls stay.)
-
+// |(x, y)| within 2 ulp of hypot (the pipelined OQPSK kernel's |sig2|). A shorter tanh, 1 - 2/(exp(2|x|)+1), made the kernels
+// slower (divergent branches), so tanh stays the library's.
 __device__ __forceinline__ double hypot_fast(double x, double y) { return sqrt(__fma_rn(x, x, y * y)); }
 
 struct Osc {                       // WaveTable (DSP.h:40-81)
@@ -218,7 +217,6 @@ __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.comm
 __device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_read_1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }   // all but the newest group
 __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-__device__ __forceinline__ void l1_prefetch(const void *p) { asm volatile("prefetch.global.L1 [%0];" ::"l"(p)); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 } // namespace jb

@@ -1,4 +1,4 @@
-// Single translation unit for the two segment kernels (they share the __constant__ tap table).
+// Single translation unit for the continuous demodulator kernels; each file also compiles on its own.
 // Built with -fmad=false: see demod_device.cuh.
 #include "oqpsk_demod.cu"
 #include "oqpsk_pipe.cu"
