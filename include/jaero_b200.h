@@ -307,6 +307,51 @@ int jaero_ingest_message(jaero_ingest *g, const void *topic, size_t topic_len, c
 size_t jaero_ingest_available(const jaero_ingest *g);                  /* samples every channel has */
 int jaero_ingest_flush(jaero_ingest *g, jaero_batch *b, size_t n_samples);
 
+/* ---- wideband IQ digital down-converter (DDC) ----
+ * Turns one complex IQ stream from a software radio (interleaved cu8 as an RTL-SDR delivers it, or cs16) into one real int16 PCM
+ * stream per channel at output rate Fs_out = input_rate / decimation, the audio input of the demodulators (Fs 48000). The PCM
+ * stays in device memory for jaero_batch_write_device / jaero_burst_write_device. Per channel c, with input x[n] counted from
+ * create (x[n<0] = 0; cu8: (v - 127.5) / 128, cs16: v / 32768), T_c = round(offset_hz[c] / input_rate * 2^32) mod 2^32 and
+ * S_c = round(audio_hz[c] / Fs_out * 2^32) mod 2^32:
+ *   z[n] = x[n] exp(-2 pi i ((n T_c) mod 2^32) / 2^32);  u[j] = sum_k h1[k] z[j D1 - k];  v[m] = sum_k h2[k] u[m D2 - k]
+ *   pcm[m] = clamp(rint(gain * 32768 * Re{v[m] exp(2 pi i ((m S_c) mod 2^32) / 2^32)}), -32768, 32767)  (rint: half to even)
+ * Output m exists once input m * decimation has arrived: N inputs give floor((N - 1) / decimation) + 1 outputs per channel, and
+ * the output does not depend on how the stream is cut into writes. After a retune, a stage-1 sample u[j] uses the offset in force
+ * when input j * D1 arrives and an output m the audio frequency in force when input m * decimation arrives.
+ * Filters (jaero_ddc_plan): real low-pass stages, h1 decimating by D1 and h2 by D2 (D1 * D2 = decimation; D2 = 1, h2 = {1} is a
+ * single stage), whose composite response passes |f| <= bandwidth/2 around the offset within +-0.1 dB of its 0 Hz gain and
+ * attenuates every tone with |f| >= bandwidth/2 + transition, up to +-input_rate/2 and aliases included, by at least 70 dB. */
+#define JAERO_IQ_CU8 0   /* interleaved unsigned 8-bit I, Q */
+#define JAERO_IQ_CS16 1  /* interleaved signed 16-bit I, Q */
+typedef struct jaero_ddc jaero_ddc;
+/* Host only, no device needed: the stages create would use, stages = {D1, K1, D2, K2} (K = number of taps); h1 [K1] and h2 [K2]
+ * receive the taps unless NULL (pass NULL to query the lengths first). */
+int jaero_ddc_plan(double input_rate, int decimation, double bandwidth, double transition, int32_t stages[4], double *h1, double *h2);
+/* Rejects a channel whose |offset_hz| exceeds input_rate/2 - bandwidth/2 or whose audio passband
+ * [audio_hz - bandwidth/2, audio_hz + bandwidth/2] leaves (0, Fs_out/2). */
+int jaero_ddc_create(double input_rate, int decimation, int n_channels, const double *offset_hz, const double *audio_hz,
+                     double bandwidth, double transition, double gain, int device_ordinal, jaero_ddc **out);
+void jaero_ddc_destroy(jaero_ddc *d);
+/* n_iq complex samples, format JAERO_IQ_*. HOST iq (copied before the call returns) */
+int jaero_ddc_write(jaero_ddc *d, const void *iq, size_t n_iq, int format);
+/* Same, iq resident in this GPU's memory (aligned to one sample) */
+int jaero_ddc_write_device(jaero_ddc *d, const void *d_iq, size_t n_iq, int format);
+/* The PCM the last write produced: d_pcm[ch * stride + i], i < n, device memory, rows 16-byte aligned (stride a multiple of 8).
+ * Valid until the next write and ordered on the DDC's stream: put the consuming batch on the same stream (jaero_batch_set_stream,
+ * jaero_ddc_set_stream). */
+int jaero_ddc_output(jaero_ddc *d, const int16_t **d_pcm, size_t *n, size_t *stride);
+/* Host copy of the same: out[ch * cap_per_channel + i]; *n = outputs per channel. Synchronises. */
+int jaero_ddc_read_pcm(jaero_ddc *d, int16_t *out, size_t cap_per_channel, size_t *n);
+/* Run on a caller-owned CUDA stream (cudaStream_t as void*; NULL = back to the DDC's own stream) */
+int jaero_ddc_set_stream(jaero_ddc *d, void *cuda_stream);
+/* Retune between writes (channel -1: every channel); same limits as create. Ordered on the DDC's stream: writes issued before
+ * the call use the old value, later writes the new one; the host does not wait. */
+int jaero_ddc_set_offset(jaero_ddc *d, int channel, double hz);
+int jaero_ddc_set_audio_freq(jaero_ddc *d, int channel, double hz);
+/* input samples written so far; clipped [n_channels] output samples clamped to the int16 range (either may be NULL) */
+int jaero_ddc_get_stats(jaero_ddc *d, int64_t *inputs, int64_t *clipped);
+int64_t jaero_ddc_launch_count(const jaero_ddc *d);
+
 /* ---- ISU / SSU reassembly and ACARS block parsing (SURVEY.md section 8(f)4, host side) ----
  * One handle per channel. Replaces RISUData::update (JAERO/aerol.cpp:27-112), ISUData::update (:151-214),
  * ParserISU::parse (:340-487) and ACARSDefragmenter (:221-329), fed the way AeroL::Decode feeds them (:1357-1399 R

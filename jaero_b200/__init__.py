@@ -12,6 +12,7 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("JAERO_B200_LIB", os.path.join(_HERE, "libjaero_b200.so"))   # override: kernel A/B experiments
 KIND_OQPSK, KIND_MSK = 0, 1
+IQ_CU8, IQ_CS16 = 0, 1
 _lib = None
 
 
@@ -67,7 +68,10 @@ EXPORTS = ["jaero_last_error", "jaero_device_count", "jaero_batch_create", "jaer
            "jaero_cchannel_tick", "jaero_cchannel_read_frames", "jaero_cchannel_get_stats", "jaero_cchannel_launch_count",
            "jaero_ingest_create", "jaero_ingest_destroy", "jaero_ingest_message", "jaero_ingest_available", "jaero_ingest_flush",
            "jaero_reasm_create", "jaero_reasm_destroy", "jaero_reasm_reset", "jaero_reasm_short_frame", "jaero_reasm_push_su",
-           "jaero_reasm_push_r", "jaero_reasm_push_t_packet", "jaero_reasm_pending", "jaero_reasm_pop", "jaero_reasm_get_stats"]
+           "jaero_reasm_push_r", "jaero_reasm_push_t_packet", "jaero_reasm_pending", "jaero_reasm_pop", "jaero_reasm_get_stats",
+           "jaero_ddc_plan", "jaero_ddc_create", "jaero_ddc_destroy", "jaero_ddc_write", "jaero_ddc_write_device", "jaero_ddc_output",
+           "jaero_ddc_read_pcm", "jaero_ddc_set_stream", "jaero_ddc_set_offset", "jaero_ddc_set_audio_freq", "jaero_ddc_get_stats",
+           "jaero_ddc_launch_count"]
 
 
 def lib():
@@ -160,6 +164,16 @@ def lib():
         L.jaero_reasm_pending.argtypes = [vp]
         L.jaero_reasm_pop.argtypes = [vp, ctypes.POINTER(AcarsRecord), vp, sz]; L.jaero_reasm_pop.restype = ctypes.c_long
         L.jaero_reasm_get_stats.argtypes = [vp, vp, vp, vp, vp]
+        L.jaero_ddc_plan.argtypes = [d, i, d, d, vp, vp, vp]
+        L.jaero_ddc_create.argtypes = [d, i, i, vp, vp, d, d, d, i, ctypes.POINTER(vp)]
+        L.jaero_ddc_destroy.argtypes = [vp]; L.jaero_ddc_destroy.restype = None
+        L.jaero_ddc_write.argtypes = [vp, vp, sz, i]; L.jaero_ddc_write_device.argtypes = [vp, vp, sz, i]
+        L.jaero_ddc_output.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(sz), ctypes.POINTER(sz)]
+        L.jaero_ddc_read_pcm.argtypes = [vp, vp, sz, ctypes.POINTER(sz)]
+        L.jaero_ddc_set_stream.argtypes = [vp, vp]
+        L.jaero_ddc_set_offset.argtypes = [vp, i, d]; L.jaero_ddc_set_audio_freq.argtypes = [vp, i, d]
+        L.jaero_ddc_get_stats.argtypes = [vp, vp, vp]
+        L.jaero_ddc_launch_count.argtypes = [vp]; L.jaero_ddc_launch_count.restype = ctypes.c_int64
         _lib = L
     return _lib
 
@@ -741,6 +755,100 @@ class Reassembler:
     def close(self):
         if self.h:
             lib().jaero_reasm_destroy(self.h); self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def ddc_plan(input_rate, decimation, bandwidth, transition):
+    """The down-converter's filter stages for a set-up (host only, no device): dict(D1, K1, D2, K2, h1, h2)."""
+    st = np.zeros(4, dtype=np.int32)
+    _check(lib().jaero_ddc_plan(float(input_rate), int(decimation), float(bandwidth), float(transition), _p(st), None, None))
+    h1 = np.zeros(int(st[1])); h2 = np.zeros(int(st[3]))
+    _check(lib().jaero_ddc_plan(float(input_rate), int(decimation), float(bandwidth), float(transition), _p(st), _p(h1), _p(h2)))
+    return dict(D1=int(st[0]), K1=int(st[1]), D2=int(st[2]), K2=int(st[3]), h1=h1, h2=h2)
+
+
+class Ddc:
+    """Wideband IQ digital down-converter (include/jaero_b200.h, jaero_ddc_*): one cu8 / cs16 IQ stream at input_rate ->
+    n_channels real int16 PCM streams at input_rate / decimation, channel c tuned to offsets_hz[c] and placed at audio_hz[c]."""
+    FORMATS = {"cu8": IQ_CU8, "cs16": IQ_CS16, IQ_CU8: IQ_CU8, IQ_CS16: IQ_CS16}
+
+    def __init__(self, input_rate, decimation, offsets_hz, audio_hz, bandwidth, transition, gain=1.0, device=0):
+        off = np.ascontiguousarray(offsets_hz, dtype=np.float64).reshape(-1)
+        if len(off) == 0:
+            raise JaeroError("at least one channel is needed")
+        aud = np.ascontiguousarray(np.broadcast_to(np.asarray(audio_hz, dtype=np.float64), off.shape))
+        self.n = len(off)
+        self.input_rate, self.decimation = float(input_rate), int(decimation)
+        self.h = ctypes.c_void_p()
+        _check(lib().jaero_ddc_create(self.input_rate, self.decimation, self.n, _p(off), _p(aud), float(bandwidth), float(transition),
+                                      float(gain), device, ctypes.byref(self.h)))
+        self.plan = ddc_plan(input_rate, decimation, bandwidth, transition)
+
+    @staticmethod
+    def _iq(iq, fmt):
+        if fmt not in Ddc.FORMATS:
+            raise ValueError("IQ format is 'cu8' or 'cs16'")
+        f = Ddc.FORMATS[fmt]
+        iq = np.ascontiguousarray(iq)
+        want = np.uint8 if f == IQ_CU8 else np.int16
+        if iq.dtype != want:
+            raise ValueError("%s IQ must be %s, got %s" % ("cu8" if f == IQ_CU8 else "cs16", np.dtype(want).name, iq.dtype))
+        if iq.size % 2:
+            raise ValueError("interleaved IQ needs an even number of values")
+        return iq, f
+
+    def write(self, iq, fmt):
+        """iq: interleaved I, Q (uint8 for 'cu8', int16 for 'cs16'), host memory"""
+        iq, f = self._iq(iq, fmt)
+        _check(lib().jaero_ddc_write(self.h, _p(iq), iq.size // 2, f))
+
+    def write_device(self, dev_ptr, n_iq, fmt):
+        if fmt not in self.FORMATS:
+            raise ValueError("IQ format is 'cu8' or 'cs16'")
+        _check(lib().jaero_ddc_write_device(self.h, ctypes.c_void_p(dev_ptr), int(n_iq), self.FORMATS[fmt]))
+
+    def output(self):
+        """(device pointer, outputs per channel, row stride) of the PCM the last write produced"""
+        a, n, s = ctypes.c_void_p(), ctypes.c_size_t(), ctypes.c_size_t()
+        _check(lib().jaero_ddc_output(self.h, ctypes.byref(a), ctypes.byref(n), ctypes.byref(s)))
+        return a.value, n.value, s.value
+
+    def read_pcm(self):
+        """host copy [n_channels, n] of the PCM the last write produced"""
+        _, n, _ = self.output()
+        out = np.zeros((self.n, max(n, 1)), dtype=np.int16)
+        got = ctypes.c_size_t()
+        _check(lib().jaero_ddc_read_pcm(self.h, _p(out), out.shape[1], ctypes.byref(got)))
+        return out[:, :got.value]
+
+    def set_stream(self, cuda_stream):
+        _check(lib().jaero_ddc_set_stream(self.h, ctypes.c_void_p(cuda_stream)))
+
+    def set_offset(self, hz, channel=-1):
+        _check(lib().jaero_ddc_set_offset(self.h, channel, float(hz)))
+
+    def set_audio_freq(self, hz, channel=-1):
+        _check(lib().jaero_ddc_set_audio_freq(self.h, channel, float(hz)))
+
+    def stats(self):
+        """(input samples written, clipped output samples per channel)"""
+        n = ctypes.c_int64()
+        clipped = np.zeros(self.n, dtype=np.int64)
+        _check(lib().jaero_ddc_get_stats(self.h, ctypes.byref(n), _p(clipped)))
+        return n.value, clipped
+
+    @property
+    def launches(self):
+        return lib().jaero_ddc_launch_count(self.h)
+
+    def close(self):
+        if self.h:
+            lib().jaero_ddc_destroy(self.h); self.h = None
 
     def __del__(self):
         try:

@@ -11,6 +11,7 @@
 #include "burst.cuh"
 #include "rtchannel.cuh"
 #include "cchannel.cuh"
+#include "ddc.cuh"
 #include <cstring>
 #include <complex>
 #include <climits>
@@ -2044,6 +2045,284 @@ int jaero_ingest_flush(jaero_ingest *g, jaero_batch *b, size_t n)
         int16_t *row = g->pcm.data() + (size_t)c * g->cap;
         memmove(row, row + n, (g->fill[c] - n) * 2);
         g->fill[c] -= n;
+    }
+    return JAERO_OK;
+}
+
+} // extern "C"
+
+// ------------------------------------------------------------------ wideband IQ down-converter
+// Filter design: Kaiser-windowed sinc, designed for DDC_DESIGN_DB of stopband attenuation (the specification asks 70 dB; the
+// margin covers the length estimate) with its cut-off half-way through the transition band and unit gain at 0 Hz. A Kaiser
+// window's passband ripple equals its stopband ripple, far inside the +-0.1 dB the specification allows.
+static const double DDC_DESIGN_DB = 76.0;
+static const int DDC_MAX_TAPS = 1 << 15;
+
+static int kaiser_length(double fs, double fpass, double fstop)
+{
+    const double dw = 2 * M_PI * (fstop - fpass) / fs;
+    const double n = (DDC_DESIGN_DB - 7.95) / (2.285 * dw) + 1.0;
+    if (!(n < DDC_MAX_TAPS)) return DDC_MAX_TAPS + 1;
+    return (int)ceil(n) | 1;                                        // odd: a whole-sample group delay
+}
+static double bessel_i0(double x)
+{
+    double s = 1.0, t = 1.0;
+    for (int k = 1; k < 200 && t > 1e-17 * s; k++) { t *= (x / (2.0 * k)) * (x / (2.0 * k)); s += t; }
+    return s;
+}
+static void kaiser_lowpass(double fs, double fpass, double fstop, int n, double *h)
+{
+    const double beta = 0.1102 * (DDC_DESIGN_DB - 8.7), fc = 0.5 * (fpass + fstop) / fs, m = 0.5 * (n - 1);
+    double sum = 0.0;
+    for (int k = 0; k < n; k++) {
+        const double t = k - m, r = m > 0 ? t / m : 0.0;
+        const double sinc = t == 0.0 ? 2 * fc : sin(2 * M_PI * fc * t) / (M_PI * t);
+        h[k] = sinc * bessel_i0(beta * sqrt(std::max(0.0, 1.0 - r * r))) / bessel_i0(beta);
+        sum += h[k];
+    }
+    for (int k = 0; k < n; k++) h[k] /= sum;
+}
+
+struct DdcPlan { int D1, K1, D2, K2; double fs1; };
+
+// The split D = D1 * D2 with the fewest multiply-adds per output (a stage-1 tap is a complex x complex product, twice a
+// stage-2 tap). Stage 1 passes B/2 and stops Fs1 - B/2 - transition, everything that would alias into stage 2's passband;
+// stage 2 passes B/2 and stops B/2 + transition.
+static int ddc_plan_stages(double fs, int D, double B, double dT, DdcPlan *out, const char *fn)
+{
+    const double fs_out = fs / D, fp = 0.5 * B, fst = 0.5 * B + dT;
+    if (!(fs > 0) || D < 1 || !(B > 0) || !(dT > 0)) { set_error(std::string(fn) + ": rates, bandwidth and transition must be positive"); return JAERO_E_ARG; }
+    if (!(fst <= 0.5 * fs_out)) { set_error(std::string(fn) + ": bandwidth/2 + transition must not exceed half the output rate"); return JAERO_E_ARG; }
+    long best = -1;
+    for (int D1 = 1; D1 <= D; D1++) {
+        if (D % D1) continue;
+        DdcPlan c{D1, 0, D / D1, 1, fs / D1};
+        if (c.D2 == 1) c.K1 = kaiser_length(fs, fp, fst);
+        else {
+            if (D1 == 1) continue;                                   // a stage 1 that does not decimate only adds work
+            c.K1 = kaiser_length(fs, fp, c.fs1 - fst);
+            c.K2 = kaiser_length(c.fs1, fp, fst);
+        }
+        if (c.K1 > DDC_MAX_TAPS || c.K2 > DDC_MAX_TAPS || (DDC_TILE_J - 1) * D1 + c.K1 > DDC_MAX_TILE) continue;
+        const long cost = 2L * c.D2 * c.K1 + c.K2;
+        if (best < 0 || cost < best) { best = cost; *out = c; }
+    }
+    if (best < 0) { set_error(std::string(fn) + ": no two-stage split of this decimation meets the filter specification within the tap limits"); return JAERO_E_ARG; }
+    return JAERO_OK;
+}
+static void ddc_design(double fs, double B, double dT, const DdcPlan &c, double *h1, double *h2)
+{
+    const double fp = 0.5 * B, fst = 0.5 * B + dT;
+    if (c.D2 == 1) { kaiser_lowpass(fs, fp, fst, c.K1, h1); h2[0] = 1.0; return; }
+    kaiser_lowpass(fs, fp, c.fs1 - fst, c.K1, h1);
+    kaiser_lowpass(c.fs1, fp, fst, c.K2, h2);
+}
+// round(f / fs * 2^32) mod 2^32
+static uint32_t tuning_word(double f, double fs) { return (uint32_t)(uint64_t)llround(f / fs * 4294967296.0); }
+
+struct jaero_ddc {
+    int device; cudaStream_t stream, own_stream;
+    std::vector<void *> allocs;
+    DdcParams p;
+    double fs_in, fs_out, B;
+    std::vector<double> h1;                                          // host copy, for re-folding on set_offset
+    std::vector<uint32_t> T, S;
+    std::vector<double2> h1c;                                        // [K1][cpad] staging for the folded taps
+    long long n_in, launches;
+    void *d_raw; size_t raw_cap;                                     // host writes: the IQ bytes staged on the device
+    double2 *d_x, *d_u; size_t x_cap, u_cap;
+    int16_t *d_pcm; size_t pcm_cap, pcm_n, pcm_stride;
+};
+
+// Retunes are ordered on the DDC's stream like its kernels: writes queued before a retune read the old values, writes after it the
+// new ones, with no wait on the host. A pageable host-to-device cudaMemcpyAsync has copied its source out of the host buffer
+// when it returns (CUDA runtime API synchronisation rules), so the host tables may change again right after.
+// The tuning words of channel c (c < 0: every channel), host words -> device words.
+static int ddc_upload_words(jaero_ddc *d, const std::vector<uint32_t> &w, const uint32_t *dev, int c)
+{
+    const size_t c0 = c < 0 ? 0 : (size_t)c, n = c < 0 ? (size_t)d->p.n_channels : 1;
+    JB_CUDA(cudaMemcpyAsync((void *)(dev + c0), w.data() + c0, n * sizeof(uint32_t), cudaMemcpyHostToDevice, d->stream));
+    return JAERO_OK;
+}
+// Folds channel c's mix into its stage-1 taps (c < 0: every channel) and uploads that channel's column of the [K1][cpad] table
+// with its tuning word.
+static int ddc_upload_offset(jaero_ddc *d, int c)
+{
+    DdcParams &p = d->p;
+    const int c0 = c < 0 ? 0 : c, c1 = c < 0 ? p.n_channels : c + 1;
+    for (int ch = c0; ch < c1; ch++)
+        for (int k = 0; k < p.K1; k++) {
+            const double th = 2 * M_PI * (double)(uint32_t)((uint32_t)k * d->T[ch]) / 4294967296.0;
+            d->h1c[(size_t)k * p.cpad + ch] = make_double2(d->h1[k] * cos(th), d->h1[k] * sin(th));
+        }
+    const size_t pitch = (size_t)p.cpad * sizeof(double2);
+    if (c < 0) JB_CUDA(cudaMemcpyAsync((void *)p.h1c, d->h1c.data(), d->h1c.size() * sizeof(double2), cudaMemcpyHostToDevice, d->stream));
+    else JB_CUDA(cudaMemcpy2DAsync((void *)(p.h1c + c), pitch, d->h1c.data() + c, pitch, sizeof(double2), p.K1, cudaMemcpyHostToDevice, d->stream));
+    return ddc_upload_words(d, d->T, p.T, c);
+}
+static bool ddc_offset_ok(const jaero_ddc *d, double hz) { return std::isfinite(hz) && fabs(hz) <= 0.5 * d->fs_in - 0.5 * d->B; }
+static bool ddc_audio_ok(const jaero_ddc *d, double hz) { return std::isfinite(hz) && hz - 0.5 * d->B > 0 && hz + 0.5 * d->B < 0.5 * d->fs_out; }
+
+extern "C" {
+
+int jaero_ddc_plan(double input_rate, int decimation, double bandwidth, double transition, int32_t stages[4], double *h1, double *h2)
+{
+    if (!stages) { set_error("jaero_ddc_plan: null argument"); return JAERO_E_ARG; }
+    DdcPlan c;
+    const int r = ddc_plan_stages(input_rate, decimation, bandwidth, transition, &c, "jaero_ddc_plan");
+    if (r) return r;
+    stages[0] = c.D1; stages[1] = c.K1; stages[2] = c.D2; stages[3] = c.K2;
+    if (h1 && h2) ddc_design(input_rate, bandwidth, transition, c, h1, h2);
+    else if (h1 || h2) {
+        std::vector<double> a(c.K1), b(c.K2);
+        ddc_design(input_rate, bandwidth, transition, c, a.data(), b.data());
+        if (h1) std::copy(a.begin(), a.end(), h1);
+        if (h2) std::copy(b.begin(), b.end(), h2);
+    }
+    return JAERO_OK;
+}
+
+int jaero_ddc_create(double input_rate, int decimation, int n_channels, const double *offset_hz, const double *audio_hz, double bandwidth,
+                     double transition, double gain, int device, jaero_ddc **out)
+{
+    if (!out || n_channels <= 0 || !offset_hz || !audio_hz || !std::isfinite(gain)) { set_error("jaero_ddc_create: bad argument"); return JAERO_E_ARG; }
+    DdcPlan c;
+    { const int r = ddc_plan_stages(input_rate, decimation, bandwidth, transition, &c, "jaero_ddc_create"); if (r) return r; }
+    const double fs_out = input_rate / decimation;
+    for (int ch = 0; ch < n_channels; ch++) {
+        if (!(std::isfinite(offset_hz[ch]) && fabs(offset_hz[ch]) <= 0.5 * input_rate - 0.5 * bandwidth)) {
+            set_error("jaero_ddc_create: channel " + std::to_string(ch) + ": |offset| must not exceed input_rate/2 - bandwidth/2"); return JAERO_E_ARG; }
+        if (!(std::isfinite(audio_hz[ch]) && audio_hz[ch] - 0.5 * bandwidth > 0 && audio_hz[ch] + 0.5 * bandwidth < 0.5 * fs_out)) {
+            set_error("jaero_ddc_create: channel " + std::to_string(ch) + ": the audio passband must lie inside (0, output_rate/2)"); return JAERO_E_ARG; }
+    }
+    CreateGuard<jaero_ddc> guard(jaero_ddc_destroy);
+    { const int e = guard.begin("jaero_ddc_create", device); if (e) return e; }
+    jaero_ddc *d = guard.obj;
+    d->own_stream = d->stream;
+    d->fs_in = input_rate; d->fs_out = fs_out; d->B = bandwidth;
+    DdcParams &p = d->p;
+    p.n_channels = n_channels; p.cpad = (n_channels + 31) & ~31;
+    p.D1 = c.D1; p.K1 = c.K1; p.D2 = c.D2; p.K2 = c.K2;
+    p.scale = gain * 32768.0;
+    d->h1.resize(c.K1);
+    std::vector<double> h2(c.K2);
+    ddc_design(input_rate, bandwidth, transition, c, d->h1.data(), h2.data());
+    d->T.resize(n_channels); d->S.resize(n_channels);
+    for (int ch = 0; ch < n_channels; ch++) { d->T[ch] = tuning_word(offset_hz[ch], input_rate); d->S[ch] = tuning_word(audio_hz[ch], fs_out); }
+    d->h1c.assign((size_t)c.K1 * p.cpad, make_double2(0.0, 0.0));
+    const size_t cp = p.cpad;
+    double2 *h1c; double *dh2; uint32_t *T, *S;
+    int rc = 0;
+    rc |= owned_alloc(d, &h1c, (size_t)c.K1 * cp); rc |= owned_alloc(d, &dh2, (size_t)c.K2);
+    rc |= owned_alloc(d, &T, cp); rc |= owned_alloc(d, &S, cp);
+    rc |= owned_alloc(d, &p.xhist, (size_t)std::max(1, c.K1 - 1)); rc |= owned_alloc(d, &p.uhist, (size_t)std::max(1, c.K2 - 1) * cp);
+    rc |= owned_alloc(d, &p.clipped, cp);
+    if (rc) return JAERO_E_CUDA;
+    p.h1c = h1c; p.h2 = dh2; p.T = T; p.S = S;
+    JB_CUDA(cudaMemcpyAsync(dh2, h2.data(), c.K2 * sizeof(double), cudaMemcpyHostToDevice, d->stream));
+    if (ddc_upload_offset(d, -1) || ddc_upload_words(d, d->S, p.S, -1)) return JAERO_E_CUDA;
+    JB_CUDA(cudaStreamSynchronize(d->stream));                       // the zeroed histories and the tables are in place
+    *out = guard.release();
+    return JAERO_OK;
+}
+void jaero_ddc_destroy(jaero_ddc *d)
+{
+    if (!d) return;
+    cudaSetDevice(d->device);
+    cudaStreamSynchronize(d->stream);
+    release(d, {d->d_raw, d->d_x, d->d_u, d->d_pcm}, {}, d->own_stream);
+}
+int64_t jaero_ddc_launch_count(const jaero_ddc *d) { return d ? d->launches : 0; }
+
+int jaero_ddc_write_device(jaero_ddc *d, const void *d_iq, size_t n, int format)
+{
+    if (!d || !d_iq) { set_error("jaero_ddc_write_device: null argument"); return JAERO_E_ARG; }
+    if (format != JAERO_IQ_CU8 && format != JAERO_IQ_CS16) { set_error("jaero_ddc_write_device: unknown IQ format"); return JAERO_E_ARG; }
+    if ((uintptr_t)d_iq & (format == JAERO_IQ_CU8 ? 1 : 3)) { set_error("jaero_ddc_write_device: IQ pointer not aligned to one sample"); return JAERO_E_ARG; }
+    if (n > ((size_t)1 << 34)) { set_error("jaero_ddc_write_device: too many samples in one write"); return JAERO_E_ARG; }
+    JB_CUDA(cudaSetDevice(d->device));
+    DdcParams &p = d->p;
+    const long long n0 = d->n_in, D = (long long)p.D1 * p.D2;
+    const size_t M = (size_t)((n0 + (long long)n + D - 1) / D - (n0 + D - 1) / D);
+    const size_t J = (size_t)((n0 + (long long)n + p.D1 - 1) / p.D1 - (n0 + p.D1 - 1) / p.D1);
+    const size_t stride = std::max<size_t>(8, (M + 7) & ~(size_t)7);   // 16-byte rows: jaero_batch_write_device reads them in place
+    if (n > 0) {
+        // a failed write leaves the output of the previous one described
+        if (grow(&d->d_x, &d->x_cap, (size_t)(p.K1 - 1) + n, d->stream) || grow(&d->d_u, &d->u_cap, ((size_t)(p.K2 - 1) + J) * p.cpad, d->stream) ||
+            grow(&d->d_pcm, &d->pcm_cap, (size_t)p.n_channels * stride, d->stream)) return JAERO_E_CUDA;
+        if (ddc_run(p, d_iq, format, n0, (long long)n, d->d_x, d->d_u, d->d_pcm, stride, d->stream, &d->launches)) return JAERO_E_CUDA;
+        d->n_in += (long long)n;
+    }
+    d->pcm_n = M; d->pcm_stride = stride;
+    return JAERO_OK;
+}
+int jaero_ddc_write(jaero_ddc *d, const void *iq, size_t n, int format)
+{
+    if (!d || !iq) { set_error("jaero_ddc_write: null argument"); return JAERO_E_ARG; }
+    if (format != JAERO_IQ_CU8 && format != JAERO_IQ_CS16) { set_error("jaero_ddc_write: unknown IQ format"); return JAERO_E_ARG; }
+    if (n > ((size_t)1 << 34)) { set_error("jaero_ddc_write: too many samples in one write"); return JAERO_E_ARG; }
+    JB_CUDA(cudaSetDevice(d->device));
+    const size_t bytes = n * (format == JAERO_IQ_CU8 ? 2 : 4);
+    if (grow((uint8_t **)&d->d_raw, &d->raw_cap, std::max<size_t>(bytes, 4), d->stream)) return JAERO_E_CUDA;
+    if (bytes) {
+        JB_CUDA(cudaMemcpyAsync(d->d_raw, iq, bytes, cudaMemcpyHostToDevice, d->stream));
+        JB_CUDA(cudaStreamSynchronize(d->stream));                   // the caller may reuse its pageable buffer on return
+    }
+    return jaero_ddc_write_device(d, d->d_raw, n, format);
+}
+int jaero_ddc_output(jaero_ddc *d, const int16_t **d_pcm, size_t *n, size_t *stride)
+{
+    if (!d || !d_pcm || !n || !stride) { set_error("jaero_ddc_output: null argument"); return JAERO_E_ARG; }
+    *d_pcm = d->d_pcm; *n = d->pcm_n; *stride = d->pcm_stride;
+    return JAERO_OK;
+}
+int jaero_ddc_read_pcm(jaero_ddc *d, int16_t *out, size_t cap, size_t *n)
+{
+    if (!d || !out || !n) { set_error("jaero_ddc_read_pcm: null argument"); return JAERO_E_ARG; }
+    if (cap < d->pcm_n) { set_error("jaero_ddc_read_pcm: cap_per_channel is smaller than the last write's output"); return JAERO_E_ARG; }
+    JB_CUDA(cudaSetDevice(d->device));
+    if (d->pcm_n)
+        JB_CUDA(cudaMemcpy2DAsync(out, cap * sizeof(int16_t), d->d_pcm, d->pcm_stride * sizeof(int16_t), d->pcm_n * sizeof(int16_t),
+                                  d->p.n_channels, cudaMemcpyDeviceToHost, d->stream));
+    JB_CUDA(cudaStreamSynchronize(d->stream));
+    *n = d->pcm_n;
+    return JAERO_OK;
+}
+int jaero_ddc_set_stream(jaero_ddc *d, void *cuda_stream)
+{
+    if (!d) { set_error("null handle"); return JAERO_E_ARG; }
+    JB_CUDA(cudaSetDevice(d->device));
+    JB_CUDA(cudaStreamSynchronize(d->stream));
+    d->stream = cuda_stream ? (cudaStream_t)cuda_stream : d->own_stream;
+    return JAERO_OK;
+}
+int jaero_ddc_set_offset(jaero_ddc *d, int channel, double hz)
+{
+    if (!d || channel < -1 || channel >= d->p.n_channels) { set_error("jaero_ddc_set_offset: bad argument"); return JAERO_E_ARG; }
+    if (!ddc_offset_ok(d, hz)) { set_error("jaero_ddc_set_offset: |offset| must not exceed input_rate/2 - bandwidth/2"); return JAERO_E_ARG; }
+    JB_CUDA(cudaSetDevice(d->device));
+    const uint32_t w = tuning_word(hz, d->fs_in);
+    for (int c = 0; c < d->p.n_channels; c++) if (channel < 0 || c == channel) d->T[c] = w;
+    return ddc_upload_offset(d, channel);
+}
+int jaero_ddc_set_audio_freq(jaero_ddc *d, int channel, double hz)
+{
+    if (!d || channel < -1 || channel >= d->p.n_channels) { set_error("jaero_ddc_set_audio_freq: bad argument"); return JAERO_E_ARG; }
+    if (!ddc_audio_ok(d, hz)) { set_error("jaero_ddc_set_audio_freq: the audio passband must lie inside (0, output_rate/2)"); return JAERO_E_ARG; }
+    JB_CUDA(cudaSetDevice(d->device));
+    const uint32_t w = tuning_word(hz, d->fs_out);
+    for (int c = 0; c < d->p.n_channels; c++) if (channel < 0 || c == channel) d->S[c] = w;
+    return ddc_upload_words(d, d->S, d->p.S, channel);
+}
+int jaero_ddc_get_stats(jaero_ddc *d, int64_t *inputs, int64_t *clipped)
+{
+    if (!d) { set_error("null handle"); return JAERO_E_ARG; }
+    if (inputs) *inputs = d->n_in;
+    if (clipped) {
+        JB_CUDA(cudaSetDevice(d->device));
+        JB_CUDA(cudaMemcpyAsync(clipped, d->p.clipped, d->p.n_channels * sizeof(int64_t), cudaMemcpyDeviceToHost, d->stream));
+        JB_CUDA(cudaStreamSynchronize(d->stream));
     }
     return JAERO_OK;
 }
