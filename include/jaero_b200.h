@@ -352,6 +352,75 @@ int jaero_ddc_set_audio_freq(jaero_ddc *d, int channel, double hz);
 int jaero_ddc_get_stats(jaero_ddc *d, int64_t *inputs, int64_t *clipped);
 int64_t jaero_ddc_launch_count(const jaero_ddc *d);
 
+/* ---- wideband carrier scanner ----
+ * Finds the carriers in the IQ stream the down-converter takes, so that its channels can be planned from the stream itself.
+ * The scanner averages the stream's power spectrum on the device; jaero_scan_find_carriers (host only) finds and measures the
+ * carriers in it. Spectrum contract:
+ *   Input: x[n] converted as the DDC converts it (cu8: (v - 127.5) / 128, cs16: v / 32768), counted from create or the last reset.
+ *   Frames: frame f is x[f * hop + n], n < nfft; it counts once its last sample has arrived. Window: periodic Hann,
+ *   w[n] = 0.5 - 0.5 cos(2 pi n / nfft). With X_f[k] = sum_n w[n] x[f hop + n] exp(-2 pi i k n / nfft) and F frames:
+ *     mean[i] = (1/F) sum_f |X_f[k]|^2 / sum_n w[n]^2,   max_hold[i] = max_f |X_f[k]|^2 / sum_n w[n]^2
+ *   in fftshift order: index i is bin k = (i + nfft/2) mod nfft, at (i - nfft/2) * input_rate / nfft Hz from the tuner centre.
+ *   Units: complex white noise of variance s^2 gives mean ~ s^2 in every bin; a carrier's mean-square power is
+ *   (1/nfft) * sum over its bins of (mean - floor). A bursty carrier shows its burst level in max_hold and is diluted by its duty
+ *   cycle in mean.
+ *   The per-frame powers are added into the running sum in frame order, so mean and max_hold are bit-identical however the
+ *   stream is cut into writes. With no frame yet, both are 0. */
+#define JAERO_MODE_UNKNOWN 0
+#define JAERO_MODE_MSK600 1
+#define JAERO_MODE_MSK1200 2
+#define JAERO_MODE_OQPSK8400 3
+#define JAERO_MODE_OQPSK10500 4
+#define JAERO_CARRIER_AT_DC 1     /* |center_hz| < dc_guard_hz: an RTL-SDR's DC spike may be all there is */
+#define JAERO_CARRIER_AT_EDGE 2   /* the run touches the first or last bin: the carrier may extend past the band */
+typedef struct jaero_scan jaero_scan;
+/* nfft a power of two from 2^10 to 2^16, 1 <= hop <= nfft, input_rate > 0. Fails with JAERO_E_CUDA without a device. */
+int jaero_scan_create(double input_rate, int nfft, int hop, int device_ordinal, jaero_scan **out);
+void jaero_scan_destroy(jaero_scan *s);
+/* n_iq complex samples, format JAERO_IQ_CU8 / JAERO_IQ_CS16. HOST iq (copied before the call returns). A failed write leaves the
+ * average unchanged. */
+int jaero_scan_write(jaero_scan *s, const void *iq, size_t n_iq, int format);
+/* Same, iq resident in this GPU's memory (aligned to one sample) */
+int jaero_scan_write_device(jaero_scan *s, const void *d_iq, size_t n_iq, int format);
+/* Run on a caller-owned CUDA stream (cudaStream_t as void*; NULL = back to the scanner's own stream) */
+int jaero_scan_set_stream(jaero_scan *s, void *cuda_stream);
+/* Start a new average: the frame count, the sample origin, mean and max_hold restart */
+int jaero_scan_reset(jaero_scan *s);
+/* mean [nfft] and max_hold [nfft] (either may be NULL), *frames = frames averaged (may be NULL). Synchronises. */
+int jaero_scan_read(jaero_scan *s, double *mean, double *max_hold, int64_t *frames);
+int64_t jaero_scan_launch_count(const jaero_scan *s);
+
+/* Carrier finding, host only (no device), on any spectrum laid out as jaero_scan_read returns it (nfft as for create, values
+ * finite and >= 0). params NULL: the defaults {3 dB, 100 kHz, 0.25, 200 Hz, 0 Hz}.
+ *   floor: W = the odd integer nearest floor_window_hz / bin_hz (2 floor(x/2) + 1), clamped to [3, nfft]; floor[i] is the order
+ *     statistic of index floor((W - 1) * floor_quantile) of psd[s .. s+W-1], s = clamp(i - (W-1)/2, 0, nfft - W). A low
+ *     quantile keeps the floor right where much of a window is occupied.
+ *   runs: bin i is occupied when psd[i] >= floor[i] * 10^(threshold_db/10); carriers are the maximal runs of occupied bins with
+ *     (bins * bin_hz) >= min_width_hz.
+ *   per run, e = psd - floor: lo_hz / hi_hz the first / last bin's frequency; peak_hz the strongest bin (largest psd, the first
+ *     on ties); center_hz the centroid of e (peak_hz if sum e <= 0); power = sum e / nfft; snr_db = 10 log10(sum e / sum floor);
+ *     peak_db = 10 log10(max psd / floor); floor = the floor at the peak bin; width_hz the half-power width of e around the peak:
+ *     with `top` the mean e of the run's bins whose e is at least half the run's largest e, from the peak outwards to the first
+ *     bin whose e is below top / 2, each crossing interpolated linearly between that bin and the one before it (the band's
+ *     first / last bin when there is none). The mean over the top, not the single largest bin, sets the level because the
+ *     largest of many noisy bins lies well above the true peak of an averaged spectrum. mode: the JAERO_MODE_* whose nominal half-power
+ *     width is nearest to width_hz on a log scale, UNKNOWN when the ratio to it is outside [0.8, 1.25].
+ * Carriers come out in ascending frequency, at most cap of them; *n_found is the total even when cap is smaller. */
+typedef struct jaero_scan_params {
+    double threshold_db;      /* > 0 */
+    double floor_window_hz;   /* > 0 */
+    double floor_quantile;    /* [0, 1] */
+    double min_width_hz;      /* >= 0 */
+    double dc_guard_hz;       /* >= 0 */
+} jaero_scan_params;
+typedef struct jaero_carrier {
+    double center_hz, peak_hz, lo_hz, hi_hz, width_hz, power, snr_db, peak_db, floor;
+    int32_t mode;             /* JAERO_MODE_* hint */
+    int32_t flags;            /* JAERO_CARRIER_* */
+} jaero_carrier;
+int jaero_scan_find_carriers(const double *psd, int nfft, double input_rate, const jaero_scan_params *params,
+                             jaero_carrier *out, int cap, int *n_found);
+
 /* ---- ISU / SSU reassembly and ACARS block parsing (SURVEY.md section 8(f)4, host side) ----
  * One handle per channel. Replaces RISUData::update (JAERO/aerol.cpp:27-112), ISUData::update (:151-214),
  * ParserISU::parse (:340-487) and ACARSDefragmenter (:221-329), fed the way AeroL::Decode feeds them (:1357-1399 R

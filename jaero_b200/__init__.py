@@ -71,7 +71,22 @@ EXPORTS = ["jaero_last_error", "jaero_device_count", "jaero_batch_create", "jaer
            "jaero_reasm_push_r", "jaero_reasm_push_t_packet", "jaero_reasm_pending", "jaero_reasm_pop", "jaero_reasm_get_stats",
            "jaero_ddc_plan", "jaero_ddc_create", "jaero_ddc_destroy", "jaero_ddc_write", "jaero_ddc_write_device", "jaero_ddc_output",
            "jaero_ddc_read_pcm", "jaero_ddc_set_stream", "jaero_ddc_set_offset", "jaero_ddc_set_audio_freq", "jaero_ddc_get_stats",
-           "jaero_ddc_launch_count"]
+           "jaero_ddc_launch_count",
+           "jaero_scan_create", "jaero_scan_destroy", "jaero_scan_write", "jaero_scan_write_device", "jaero_scan_set_stream",
+           "jaero_scan_reset", "jaero_scan_read", "jaero_scan_launch_count", "jaero_scan_find_carriers"]
+MODES = {0: "unknown", 1: "msk600", 2: "msk1200", 3: "oqpsk8400", 4: "oqpsk10500"}
+CARRIER_AT_DC, CARRIER_AT_EDGE = 1, 2
+
+
+class ScanParams(ctypes.Structure):
+    """jaero_scan_params (include/jaero_b200.h)."""
+    _fields_ = [(n, ctypes.c_double) for n in ("threshold_db", "floor_window_hz", "floor_quantile", "min_width_hz", "dc_guard_hz")]
+
+
+class Carrier(ctypes.Structure):
+    """jaero_carrier (include/jaero_b200.h)."""
+    _fields_ = [(n, ctypes.c_double) for n in ("center_hz", "peak_hz", "lo_hz", "hi_hz", "width_hz", "power", "snr_db", "peak_db",
+                                                "floor")] + [("mode", ctypes.c_int32), ("flags", ctypes.c_int32)]
 
 
 def lib():
@@ -174,6 +189,14 @@ def lib():
         L.jaero_ddc_set_offset.argtypes = [vp, i, d]; L.jaero_ddc_set_audio_freq.argtypes = [vp, i, d]
         L.jaero_ddc_get_stats.argtypes = [vp, vp, vp]
         L.jaero_ddc_launch_count.argtypes = [vp]; L.jaero_ddc_launch_count.restype = ctypes.c_int64
+        L.jaero_scan_create.argtypes = [d, i, i, i, ctypes.POINTER(vp)]
+        L.jaero_scan_destroy.argtypes = [vp]; L.jaero_scan_destroy.restype = None
+        L.jaero_scan_write.argtypes = [vp, vp, sz, i]; L.jaero_scan_write_device.argtypes = [vp, vp, sz, i]
+        L.jaero_scan_set_stream.argtypes = [vp, vp]
+        L.jaero_scan_reset.argtypes = [vp]
+        L.jaero_scan_read.argtypes = [vp, vp, vp, vp]
+        L.jaero_scan_launch_count.argtypes = [vp]; L.jaero_scan_launch_count.restype = ctypes.c_int64
+        L.jaero_scan_find_carriers.argtypes = [vp, i, d, ctypes.POINTER(ScanParams), vp, i, ctypes.POINTER(i)]
         _lib = L
     return _lib
 
@@ -855,3 +878,107 @@ class Ddc:
             self.close()
         except Exception:
             pass
+
+
+class Scanner:
+    """Wideband carrier scanner (include/jaero_b200.h, jaero_scan_*): the averaged and max-held power spectrum of one cu8 / cs16 IQ
+    stream at input_rate, nfft bins in fftshift order, frames every `hop` samples (default nfft // 2)."""
+
+    def __init__(self, input_rate, nfft, hop=None, device=0):
+        self.input_rate, self.nfft = float(input_rate), int(nfft)
+        self.hop = self.nfft // 2 if hop is None else int(hop)
+        self.h = ctypes.c_void_p()
+        _check(lib().jaero_scan_create(self.input_rate, self.nfft, self.hop, device, ctypes.byref(self.h)))
+
+    def write(self, iq, fmt):
+        """iq: interleaved I, Q (uint8 for 'cu8', int16 for 'cs16'), host memory"""
+        iq, f = Ddc._iq(iq, fmt)
+        _check(lib().jaero_scan_write(self.h, _p(iq), iq.size // 2, f))
+
+    def write_device(self, dev_ptr, n_iq, fmt):
+        if fmt not in Ddc.FORMATS:
+            raise ValueError("IQ format is 'cu8' or 'cs16'")
+        _check(lib().jaero_scan_write_device(self.h, ctypes.c_void_p(dev_ptr), int(n_iq), Ddc.FORMATS[fmt]))
+
+    def reset(self):
+        _check(lib().jaero_scan_reset(self.h))
+
+    def read(self):
+        """(mean [nfft], max_hold [nfft], frames averaged)"""
+        mean = np.zeros(self.nfft); mx = np.zeros(self.nfft); fr = ctypes.c_int64()
+        _check(lib().jaero_scan_read(self.h, _p(mean), _p(mx), ctypes.byref(fr)))
+        return mean, mx, fr.value
+
+    def freqs(self):
+        """frequency of each bin, Hz from the tuner centre"""
+        return (np.arange(self.nfft) - self.nfft // 2) * (self.input_rate / self.nfft)
+
+    def set_stream(self, cuda_stream):
+        _check(lib().jaero_scan_set_stream(self.h, ctypes.c_void_p(cuda_stream)))
+
+    @property
+    def launches(self):
+        return lib().jaero_scan_launch_count(self.h)
+
+    def close(self):
+        if self.h:
+            lib().jaero_scan_destroy(self.h); self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def find_carriers(psd, input_rate, threshold_db=3.0, floor_window_hz=100e3, floor_quantile=0.25, min_width_hz=200.0, dc_guard_hz=0.0):
+    """Carriers in a spectrum laid out as Scanner.read returns it (host only, no device; include/jaero_b200.h,
+    jaero_scan_find_carriers): a list of dicts with the fields of jaero_carrier, in ascending frequency, mode as a string."""
+    psd = np.ascontiguousarray(psd, dtype=np.float64)
+    prm = ScanParams(threshold_db, floor_window_hz, floor_quantile, min_width_hz, dc_guard_hz)
+    n = ctypes.c_int()
+    _check(lib().jaero_scan_find_carriers(_p(psd), len(psd), float(input_rate), ctypes.byref(prm), None, 0, ctypes.byref(n)))
+    arr = (Carrier * max(n.value, 1))()
+    _check(lib().jaero_scan_find_carriers(_p(psd), len(psd), float(input_rate), ctypes.byref(prm), ctypes.cast(arr, ctypes.c_void_p),
+                                          n.value, ctypes.byref(n)))
+    out = []
+    for c in arr[:n.value]:
+        d = {f[0]: getattr(c, f[0]) for f in Carrier._fields_}
+        d["mode"] = MODES[c.mode]
+        out.append(d)
+    return out
+
+
+# Down-converter and demodulator settings per continuous mode: the DDC bandwidth / transition and audio centre the end-to-end tests
+# use, and the demodulators' freq_center / lockingbw of the recordings' fixtures (48 kHz audio).
+CHANNEL_SETTINGS = {
+    "oqpsk10500": dict(kind="oqpsk", fb=10500, audio_hz=8000.0, bandwidth=12000.0, transition=4000.0, lockingbw=10500.0),
+    "oqpsk8400": dict(kind="oqpsk", fb=8400, audio_hz=8000.0, bandwidth=12000.0, transition=4000.0, lockingbw=10500.0),
+    "msk1200": dict(kind="msk", fb=1200, audio_hz=2000.0, bandwidth=3000.0, transition=1000.0, lockingbw=1800.0),
+    "msk600": dict(kind="msk", fb=600, audio_hz=1000.0, bandwidth=1500.0, transition=500.0, lockingbw=900.0),
+}
+
+
+def channel_plan(carriers, input_rate, decimation):
+    """Groups find_carriers' detections by mode into down-converter and demodulator arguments.
+
+    -> (plans, unplanned). plans[mode] = dict(ddc=kwargs of Ddc, demod=kwargs of DemodBatch, carriers=the group's detections), one
+    per continuous mode found, channels in ascending frequency. The gain puts the group's strongest carrier at 0.2 sqrt(2) rms of
+    full scale. unplanned: the carriers of unknown mode, those flagged AT_DC, and those too close to the band edge to tune."""
+    plans, unplanned = {}, []
+    for c in sorted(carriers, key=lambda c: c["center_hz"]):
+        s = CHANNEL_SETTINGS.get(c["mode"])
+        if s is None or (c["flags"] & CARRIER_AT_DC) or abs(c["center_hz"]) > input_rate / 2 - s["bandwidth"] / 2:
+            unplanned.append(c)
+        else:
+            plans.setdefault(c["mode"], []).append(c)
+    out = {}
+    for mode, group in plans.items():
+        s = CHANNEL_SETTINGS[mode]
+        gain = 0.2 * np.sqrt(2) / np.sqrt(max(c["power"] for c in group))
+        out[mode] = dict(
+            ddc=dict(input_rate=float(input_rate), decimation=int(decimation), offsets_hz=[c["center_hz"] for c in group],
+                     audio_hz=s["audio_hz"], bandwidth=s["bandwidth"], transition=s["transition"], gain=float(gain)),
+            demod=dict(kind=s["kind"], n_channels=len(group), fb=s["fb"], freq_center=s["audio_hz"], lockingbw=s["lockingbw"]),
+            carriers=group)
+    return out, unplanned

@@ -20,6 +20,7 @@ UNITS = [
     ("cchannel.cu", []),
     ("reassembly.cu", []),
     ("ddc.cu", []),
+    ("scan.cu", []),
     ("prefilter.cu", ["-fmad=false"]),
     ("burst.cu", ["-fmad=false"]),
     ("demod_kernels.cu", ["-fmad=false"]),

@@ -12,6 +12,7 @@
 #include "rtchannel.cuh"
 #include "cchannel.cuh"
 #include "ddc.cuh"
+#include "scan.cuh"
 #include <cstring>
 #include <complex>
 #include <climits>
@@ -2328,3 +2329,251 @@ int jaero_ddc_get_stats(jaero_ddc *d, int64_t *inputs, int64_t *clipped)
 }
 
 } // extern "C"
+
+// ------------------------------------------------------------------ wideband carrier scanner
+struct jaero_scan {
+    int device; cudaStream_t stream, own_stream;
+    std::vector<void *> allocs;
+    ScanPlan p;
+    long long n_in, frames, launches;                                 // samples and complete frames since create / reset
+    double2 *d_carry;                                                // [nfft] samples frames * hop .. n_in - 1 (fewer than nfft)
+    void *d_raw; size_t raw_cap;                                     // host writes: the IQ bytes staged on the device
+    double2 *d_x, *d_work; double *d_pw; size_t x_cap, work_cap, pw_cap;
+};
+
+static bool pow2_nfft(int nfft) { return nfft >= 1024 && nfft <= 65536 && (nfft & (nfft - 1)) == 0; }
+
+extern "C" {
+
+int jaero_scan_create(double input_rate, int nfft, int hop, int device, jaero_scan **out)
+{
+    if (!out) { set_error("jaero_scan_create: null argument"); return JAERO_E_ARG; }
+    if (!pow2_nfft(nfft)) { set_error("jaero_scan_create: nfft must be a power of two from 1024 to 65536"); return JAERO_E_ARG; }
+    if (hop < 1 || hop > nfft) { set_error("jaero_scan_create: hop must be in [1, nfft]"); return JAERO_E_ARG; }
+    if (!(input_rate > 0) || !std::isfinite(input_rate)) { set_error("jaero_scan_create: input_rate must be positive"); return JAERO_E_ARG; }
+    CreateGuard<jaero_scan> guard(jaero_scan_destroy);
+    { const int e = guard.begin("jaero_scan_create", device); if (e) return e; }
+    jaero_scan *s = guard.obj;
+    s->own_stream = s->stream;
+    ScanPlan &p = s->p;
+    p.nfft = nfft; p.hop = hop;
+    int lg = 0;
+    while ((1 << lg) < nfft) lg++;
+    p.n1 = 1 << (lg / 2); p.n2 = nfft / p.n1;
+    std::vector<double2> tw(nfft);
+    std::vector<double> win(nfft);
+    double wss = 0.0;
+    for (int k = 0; k < nfft; k++) {
+        const double a = 2 * M_PI * (double)k / nfft;
+        tw[k] = make_double2(cos(a), -sin(a));
+        win[k] = 0.5 - 0.5 * cos(a);
+        wss += win[k] * win[k];
+    }
+    p.inv_wss = 1.0 / wss;
+    double2 *dtw; double *dwin;
+    int rc = 0;
+    rc |= owned_alloc(s, &dtw, (size_t)nfft); rc |= owned_alloc(s, &dwin, (size_t)nfft);
+    rc |= owned_alloc(s, &p.sum, (size_t)nfft); rc |= owned_alloc(s, &p.maxh, (size_t)nfft);
+    rc |= owned_alloc(s, &s->d_carry, (size_t)nfft);
+    if (rc) return JAERO_E_CUDA;
+    p.tw = dtw; p.win = dwin;
+    JB_CUDA(cudaMemcpyAsync(dtw, tw.data(), nfft * sizeof(double2), cudaMemcpyHostToDevice, s->stream));
+    JB_CUDA(cudaMemcpyAsync(dwin, win.data(), nfft * sizeof(double), cudaMemcpyHostToDevice, s->stream));
+    JB_CUDA(cudaStreamSynchronize(s->stream));                       // the tables are in place, the host vectors may go
+    *out = guard.release();
+    return JAERO_OK;
+}
+void jaero_scan_destroy(jaero_scan *s)
+{
+    if (!s) return;
+    cudaSetDevice(s->device);
+    cudaStreamSynchronize(s->stream);
+    release(s, {s->d_raw, s->d_x, s->d_work, s->d_pw}, {}, s->own_stream);
+}
+int64_t jaero_scan_launch_count(const jaero_scan *s) { return s ? s->launches : 0; }
+
+int jaero_scan_write_device(jaero_scan *s, const void *d_iq, size_t n, int format)
+{
+    if (!s || !d_iq) { set_error("jaero_scan_write_device: null argument"); return JAERO_E_ARG; }
+    if (format != JAERO_IQ_CU8 && format != JAERO_IQ_CS16) { set_error("jaero_scan_write_device: unknown IQ format"); return JAERO_E_ARG; }
+    if ((uintptr_t)d_iq & (format == JAERO_IQ_CU8 ? 1 : 3)) { set_error("jaero_scan_write_device: IQ pointer not aligned to one sample"); return JAERO_E_ARG; }
+    if (n > ((size_t)1 << 34)) { set_error("jaero_scan_write_device: too many samples in one write"); return JAERO_E_ARG; }
+    if (n == 0) return JAERO_OK;
+    JB_CUDA(cudaSetDevice(s->device));
+    const ScanPlan &p = s->p;
+    const long long N = p.nfft, hop = p.hop, total = s->n_in + (long long)n;
+    const long long x0 = s->frames * hop, carry = s->n_in - x0;      // xd[j] = sample x0 + j
+    const long long f_end = total >= N ? (total - N) / hop + 1 : 0, F = f_end - s->frames;
+    const int G = (int)std::max<long long>(1, SCAN_PASS_ELEMS / N);
+    const size_t g = (size_t)std::min<long long>(std::max<long long>(F, 1), G);
+    // every buffer is in place before anything is queued: a failed write leaves the average unchanged
+    if (grow(&s->d_x, &s->x_cap, (size_t)(carry + (long long)n), s->stream) || grow(&s->d_work, &s->work_cap, g * N, s->stream) ||
+        grow(&s->d_pw, &s->pw_cap, g * N, s->stream)) return JAERO_E_CUDA;
+    if (carry) JB_CUDA(cudaMemcpyAsync(s->d_x, s->d_carry, carry * sizeof(double2), cudaMemcpyDeviceToDevice, s->stream));
+    if (scan_convert(d_iq, format, (long long)n, s->d_x + carry, s->stream, &s->launches)) return JAERO_E_CUDA;
+    if (F > 0 && scan_frames(p, s->d_x, x0, s->frames, F, G, s->d_work, s->d_pw, s->stream, &s->launches)) return JAERO_E_CUDA;
+    const long long x1 = f_end * hop;                                // the first sample an incomplete frame needs
+    if (total > x1) JB_CUDA(cudaMemcpyAsync(s->d_carry, s->d_x + (x1 - x0), (total - x1) * sizeof(double2), cudaMemcpyDeviceToDevice, s->stream));
+    s->n_in = total; s->frames = f_end;
+    return JAERO_OK;
+}
+int jaero_scan_write(jaero_scan *s, const void *iq, size_t n, int format)
+{
+    if (!s || !iq) { set_error("jaero_scan_write: null argument"); return JAERO_E_ARG; }
+    if (format != JAERO_IQ_CU8 && format != JAERO_IQ_CS16) { set_error("jaero_scan_write: unknown IQ format"); return JAERO_E_ARG; }
+    if (n > ((size_t)1 << 34)) { set_error("jaero_scan_write: too many samples in one write"); return JAERO_E_ARG; }
+    JB_CUDA(cudaSetDevice(s->device));
+    const size_t bytes = n * (format == JAERO_IQ_CU8 ? 2 : 4);
+    if (grow((uint8_t **)&s->d_raw, &s->raw_cap, std::max<size_t>(bytes, 4), s->stream)) return JAERO_E_CUDA;
+    if (bytes) {
+        JB_CUDA(cudaMemcpyAsync(s->d_raw, iq, bytes, cudaMemcpyHostToDevice, s->stream));
+        JB_CUDA(cudaStreamSynchronize(s->stream));                   // the caller may reuse its pageable buffer on return
+    }
+    return jaero_scan_write_device(s, s->d_raw, n, format);
+}
+int jaero_scan_set_stream(jaero_scan *s, void *cuda_stream)
+{
+    if (!s) { set_error("null handle"); return JAERO_E_ARG; }
+    JB_CUDA(cudaSetDevice(s->device));
+    JB_CUDA(cudaStreamSynchronize(s->stream));
+    s->stream = cuda_stream ? (cudaStream_t)cuda_stream : s->own_stream;
+    return JAERO_OK;
+}
+int jaero_scan_reset(jaero_scan *s)
+{
+    if (!s) { set_error("null handle"); return JAERO_E_ARG; }
+    JB_CUDA(cudaSetDevice(s->device));
+    JB_CUDA(cudaMemsetAsync(s->p.sum, 0, s->p.nfft * sizeof(double), s->stream));
+    JB_CUDA(cudaMemsetAsync(s->p.maxh, 0, s->p.nfft * sizeof(double), s->stream));
+    s->n_in = 0; s->frames = 0;
+    return JAERO_OK;
+}
+int jaero_scan_read(jaero_scan *s, double *mean, double *max_hold, int64_t *frames)
+{
+    if (!s) { set_error("null handle"); return JAERO_E_ARG; }
+    JB_CUDA(cudaSetDevice(s->device));
+    const int N = s->p.nfft;
+    if (mean) JB_CUDA(cudaMemcpyAsync(mean, s->p.sum, N * sizeof(double), cudaMemcpyDeviceToHost, s->stream));
+    if (max_hold) JB_CUDA(cudaMemcpyAsync(max_hold, s->p.maxh, N * sizeof(double), cudaMemcpyDeviceToHost, s->stream));
+    JB_CUDA(cudaStreamSynchronize(s->stream));
+    if (mean && s->frames > 0)
+        for (int i = 0; i < N; i++) mean[i] /= (double)s->frames;
+    if (frames) *frames = s->frames;
+    return JAERO_OK;
+}
+
+} // extern "C"
+
+// Carrier finding (host only). The sliding order statistic of the floor: the bins are ranked once by (value, index), a Fenwick tree
+// over the ranks holds the window's members, and the k-th smallest member is found by descending the tree, O(log nfft) per bin.
+static void scan_floor(const double *psd, int n, int W, double q, double *floor_out)
+{
+    std::vector<int> order(n), rank(n), tree(n + 1, 0);
+    for (int i = 0; i < n; i++) order[i] = i;
+    std::sort(order.begin(), order.end(), [psd](int a, int b) { return psd[a] < psd[b] || (psd[a] == psd[b] && a < b); });
+    for (int r = 0; r < n; r++) rank[order[r]] = r;
+    int top = 1;
+    while (top * 2 <= n) top *= 2;
+    auto add = [&](int bin, int d) { for (int j = rank[bin] + 1; j <= n; j += j & -j) tree[j] += d; };
+    auto kth = [&](int k) {                                          // rank of the k-th smallest member, k from 0
+        int pos = 0;
+        for (int step = top; step; step >>= 1)
+            if (pos + step <= n && tree[pos + step] <= k) { pos += step; k -= tree[pos]; }
+        return pos;
+    };
+    const int k = (int)std::floor((W - 1) * q);
+    for (int j = 0; j < W; j++) add(j, 1);
+    int s_cur = 0;
+    for (int i = 0; i < n; i++) {
+        const int s = std::min(std::max(i - (W - 1) / 2, 0), n - W);
+        for (; s_cur < s; s_cur++) { add(s_cur, -1); add(s_cur + W, 1); }
+        floor_out[i] = psd[order[kth(k)]];
+    }
+}
+
+// Nominal half-power widths of the continuous modes.
+//   OQPSK with root-raised-cosine pulses on each arm: the spectrum is a raised cosine of the symbol rate Rs = fb / 2, and a raised
+//   cosine of any roll-off is at half its peak at +-Rs/2, so the half-power width is Rs: 5250 Hz at 10500 bps, 4200 Hz at 8400.
+//   MSK with half-sine pulses: S(f) ~ [cos(2 pi f T) / (1 - 16 f^2 T^2)]^2 with T = 1 / fb falls to half its peak at
+//   f T = 0.297241, a half-power width of 0.594482 fb: 356.7 Hz at 600 bps and 713.4 Hz at 1200.
+static int scan_mode_hint(double width)
+{
+    static const double nominal[4] = {0.594482 * 600, 0.594482 * 1200, 4200.0, 5250.0};
+    static const int modes[4] = {JAERO_MODE_MSK600, JAERO_MODE_MSK1200, JAERO_MODE_OQPSK8400, JAERO_MODE_OQPSK10500};
+    if (!(width > 0)) return JAERO_MODE_UNKNOWN;
+    int best = 0;
+    for (int m = 1; m < 4; m++)
+        if (fabs(log(width / nominal[m])) < fabs(log(width / nominal[best]))) best = m;
+    const double r = width / nominal[best];
+    return (r >= 0.8 && r <= 1.25) ? modes[best] : JAERO_MODE_UNKNOWN;
+}
+
+extern "C" int jaero_scan_find_carriers(const double *psd, int nfft, double input_rate, const jaero_scan_params *params,
+                                        jaero_carrier *out, int cap, int *n_found)
+{
+    if (!psd || !n_found || (cap > 0 && !out) || cap < 0) { set_error("jaero_scan_find_carriers: bad argument"); return JAERO_E_ARG; }
+    if (!pow2_nfft(nfft)) { set_error("jaero_scan_find_carriers: nfft must be a power of two from 1024 to 65536"); return JAERO_E_ARG; }
+    if (!(input_rate > 0) || !std::isfinite(input_rate)) { set_error("jaero_scan_find_carriers: input_rate must be positive"); return JAERO_E_ARG; }
+    const jaero_scan_params P = params ? *params : jaero_scan_params{3.0, 100e3, 0.25, 200.0, 0.0};
+    if (!(P.threshold_db > 0) || !std::isfinite(P.threshold_db) || !(P.floor_window_hz > 0) || !std::isfinite(P.floor_window_hz) ||
+        !(P.floor_quantile >= 0 && P.floor_quantile <= 1) || !(P.min_width_hz >= 0) || !std::isfinite(P.min_width_hz) ||
+        !(P.dc_guard_hz >= 0) || !std::isfinite(P.dc_guard_hz)) {
+        set_error("jaero_scan_find_carriers: parameter out of range"); return JAERO_E_ARG; }
+    for (int i = 0; i < nfft; i++)
+        if (!(psd[i] >= 0) || !std::isfinite(psd[i])) { set_error("jaero_scan_find_carriers: spectrum values must be finite and >= 0"); return JAERO_E_ARG; }
+    const int n = nfft;
+    const double bin_hz = input_rate / n;
+    const double x = std::min(P.floor_window_hz / bin_hz, (double)n);
+    const int W = std::min(std::max(2 * (int)std::floor(x / 2) + 1, 3), n);
+    std::vector<double> fl(n), e(n);
+    scan_floor(psd, n, W, P.floor_quantile, fl.data());
+    for (int i = 0; i < n; i++) e[i] = psd[i] - fl[i];
+    const double thr = pow(10.0, P.threshold_db / 10.0);
+    auto hz = [&](double i) { return (i - n / 2) * bin_hz; };
+    int found = 0;
+    for (int i0 = 0; i0 < n;) {
+        if (!(psd[i0] >= fl[i0] * thr)) { i0++; continue; }
+        int i1 = i0;
+        while (i1 + 1 < n && psd[i1 + 1] >= fl[i1 + 1] * thr) i1++;
+        if ((i1 - i0 + 1) * bin_hz >= P.min_width_hz) {
+            int pk = i0;
+            double se = 0, sfe = 0, sf = 0, pr = 0, emax = e[i0];
+            for (int i = i0; i <= i1; i++) {
+                if (psd[i] > psd[pk]) pk = i;
+                se += e[i]; sfe += hz(i) * e[i]; sf += fl[i];
+                pr = std::max(pr, psd[i] / fl[i]);
+                emax = std::max(emax, e[i]);
+            }
+            // The half-power level is half the mean excess over the carrier's top (its bins at or above half the largest excess),
+            // not half the largest excess: the largest of many noisy bins sits well above the spectrum's true peak (+15 % for a
+            // 10.5 kbps carrier averaged over 300 frames), which would narrow every width and move 10.5 kbps carriers to 8400.
+            double top = 0;
+            int ntop = 0;
+            for (int i = i0; i <= i1; i++)
+                if (e[i] >= 0.5 * emax) { top += e[i]; ntop++; }
+            const double h = 0.5 * (top / ntop);
+            int j = pk + 1;
+            while (j < n && e[j] >= h) j++;
+            const double xr = j == n ? n - 1 : (j - 1) + (e[j - 1] - h) / (e[j - 1] - e[j]);
+            j = pk - 1;
+            while (j >= 0 && e[j] >= h) j--;
+            const double xl = j < 0 ? 0 : (j + 1) - (e[j + 1] - h) / (e[j + 1] - e[j]);
+            jaero_carrier c;
+            c.peak_hz = hz(pk);
+            c.center_hz = se > 0 ? sfe / se : c.peak_hz;
+            c.lo_hz = hz(i0); c.hi_hz = hz(i1);
+            c.width_hz = (xr - xl) * bin_hz;
+            c.power = se / n;
+            c.snr_db = 10 * log10(se / sf);
+            c.peak_db = 10 * log10(pr);
+            c.floor = fl[pk];
+            c.mode = scan_mode_hint(c.width_hz);
+            c.flags = (fabs(c.center_hz) < P.dc_guard_hz ? JAERO_CARRIER_AT_DC : 0) | (i0 == 0 || i1 == n - 1 ? JAERO_CARRIER_AT_EDGE : 0);
+            if (found < cap) out[found] = c;
+            found++;
+        }
+        i0 = i1 + 1;
+    }
+    *n_found = found;
+    return JAERO_OK;
+}

@@ -20,16 +20,6 @@
 
 namespace jb {
 
-__device__ __forceinline__ double2 iq_sample(const void *raw, long long i, int format)
-{
-    if (format == JAERO_IQ_CU8) {
-        const uchar2 v = reinterpret_cast<const uchar2 *>(raw)[i];
-        return make_double2(((double)v.x - 127.5) * (1.0 / 128.0), ((double)v.y - 127.5) * (1.0 / 128.0));
-    }
-    const short2 v = reinterpret_cast<const short2 *>(raw)[i];
-    return make_double2((double)v.x * (1.0 / 32768.0), (double)v.y * (1.0 / 32768.0));
-}
-
 // exp(sign * 2 pi i w / 2^32)
 __device__ __forceinline__ double2 phasor(uint32_t w)
 {

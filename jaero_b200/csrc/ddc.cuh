@@ -2,8 +2,20 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>
+#include "../../include/jaero_b200.h"
 
 namespace jb {
+
+// Raw IQ sample i of a cu8 / cs16 stream as a complex double (the carrier scanner converts its input the same way)
+__device__ __forceinline__ double2 iq_sample(const void *raw, long long i, int format)
+{
+    if (format == JAERO_IQ_CU8) {
+        const uchar2 v = reinterpret_cast<const uchar2 *>(raw)[i];
+        return make_double2(((double)v.x - 127.5) * (1.0 / 128.0), ((double)v.y - 127.5) * (1.0 / 128.0));
+    }
+    const short2 v = reinterpret_cast<const short2 *>(raw)[i];
+    return make_double2((double)v.x * (1.0 / 32768.0), (double)v.y * (1.0 / 32768.0));
+}
 
 static const int DDC_WARP_J = 8;            // stage-1 outputs one thread accumulates (register blocking over j)
 static const int DDC_WARPS = 4;             // warps of a stage-1 CTA; all of them share the CTA's 32 channels
