@@ -218,12 +218,13 @@ cfe_search_kernel(CfePlan pl, DemodParams p)
 // 128 x 128 working matrix (256 KB of complex doubles) in the distributed shared memory of its CTAs through all three
 // transforms: CTA q holds 16 columns (column passes) or 16 rows (row passes); the three layout changes are pulls from
 // the peers' shared memory (DSMEM) with the four-step twiddle folded into the pull. A CTA needs 74 KB of shared memory
-// and 256 threads, so three clusters' CTAs share an SM and three channels are in flight per SM: one channel's barrier /
-// pull latency is covered by the others' butterflies. HBM traffic per channel falls to the ring read (256 KB) plus the
+// and 128 threads; two clusters' CTAs share an SM, so one channel's barrier / pull latency is covered by the other's
+// butterflies (a third CTA would fit the shared memory, but its 168-register cap makes the kernel spill, which measured
+// slower on H100). HBM traffic per channel falls to the ring read (256 KB) plus the
 // read-modify-write of y (2 x 128 KB), from eight 256 KB matrix passes before.
 namespace cgx = cooperative_groups;
 
-static const int CC_CL = 8, CC_T = 256, CC_SEQ = 16, CC_RS = 143;             // cluster size, threads, sequences per CTA, row stride
+static const int CC_CL = 8, CC_T = 128, CC_SEQ = 16, CC_RS = 143;             // cluster size, threads, sequences per CTA, row stride
 static const int CC_BUF = CC_SEQ * CC_RS * 16;                                // one working buffer (bytes)
 static const int CC_TW2 = 128, CC_TW3 = 152;                                  // offsets (in double2) of the per-pass twiddle copies
 static const int CC_SM_TOTAL = 2 * CC_BUF + (128 + 24 + 32) * 16;
@@ -258,59 +259,71 @@ __device__ __forceinline__ double log10_ge1(double x)
     return (dk * log10_2lo + ivln10 * lg) + dk * log10_2hi;
 }
 
-// 16 x FFT-128 in place (same factorisation and arithmetic as tile_fft for n = 128: Stockham radix 8, 4, 4). Warp w owns
-// sequences w and w+8 through all three passes, so the passes are ordered by __syncwarp() only: each pass reads its
-// butterflies' inputs into registers, __syncwarp, writes the outputs back into the same rows. `last` receives
-// (sequence, position, value) of the final pass and normally stores it back (mask / square are fused there).
-// FIRST = false: the caller has already run the first (radix-8) pass from registers — the values it pulled from the ring or
-// from its peers are exactly one butterfly's inputs — stored the outputs (row[8j + t]) and passed a __syncthreads().
-template <bool INV, bool FIRST, class Store>
-__device__ __forceinline__ void cc_fft(double2 *__restrict__ buf, const double2 *__restrict__ tws, Store last)
+// 16 x FFT-128 (same factorisation and arithmetic as tile_fft for n = 128: Stockham radix 8, 4, 4), with the passes after the
+// first one in registers. Pass 2 (radix 4, Ns = 8) butterfly 8m + k writes positions 32m + k + 8t and pass 3 (radix 4, Ns = 32)
+// butterfly k + 8u reads positions k + 8u + 32i: for each k in 0..7 both passes close over the 16 positions k + 8p of the
+// sequence. Lane k of sequence f = threadIdx.x >> 3 holds those 16 values (x[p] = position k + 8p) and runs both passes without
+// touching shared memory; a warp owns four whole sequences, so only __syncwarp() orders lanes of a sequence. Pass 3 leaves
+// position k + 8p in x[p] again, and those are the inputs of the next transform's first-pass (radix 8, Ns = 1) butterflies
+// k (positions k + 16t = x[2t]) and k + 8 (x[2t + 1]): a transform chained to another is stored once, after that first pass.
+// The first pass of a transform that starts from the ring or from the peers' buffers runs from the registers of the load /
+// pull, whose eight values are exactly one butterfly's inputs.
+__device__ __forceinline__ void cc_load16(const double2 *row, int k, double2 (&x)[16])
 {
-    const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
-    if (FIRST) {   // radix 8, Ns = 1: lanes 0-15 -> sequence w, lanes 16-31 -> sequence w+8
-        double2 *row = buf + (w + ((l & 16) >> 1)) * CC_RS;
-        const int j = l & 15;
-        double2 v[8];
 #pragma unroll
-        for (int t = 0; t < 8; t++) v[t] = row[cc_ph(j + 16 * t)];
-        __syncwarp();
-        dft8<INV>(v);
+    for (int p = 0; p < 16; p++) x[p] = row[cc_ph(k + 8 * p)];
+}
+
+__device__ __forceinline__ void cc_store16(double2 *row, int k, const double2 (&x)[16])
+{
 #pragma unroll
-        for (int t = 0; t < 8; t++) row[cc_ph(8 * j + t)] = v[t];
-        __syncwarp();
-    }
-    double2 *r0 = buf + w * CC_RS, *r1 = buf + (w + 8) * CC_RS;
+    for (int p = 0; p < 16; p++) row[cc_ph(k + 8 * p)] = x[p];
+}
+
+template <bool INV>
+__device__ __forceinline__ void cc_pass23(double2 (&x)[16], int k, const double2 *__restrict__ tws)
+{
     // The twiddles of a pass depend on the lane only. Read straight from the 128-entry table the second pass's strides
     // (4k, 8k, 12k) put a quarter-warp's eight 16-byte loads on two, one and two bank groups (4-, 8- and 4-way conflicts) and
     // the third pass's 2l on four (2-way); the kernel keeps compact copies instead: tws[CC_TW2 + 8(m-1) + k] = W^(4mk),
     // tws[CC_TW3 + l] = W^(2l). Same table values, so the arithmetic is unchanged.
-    auto radix4 = [&](double2 &v0, double2 &v1, double2 &v2, double2 &v3, double2 w1, double2 w2, double2 w3) {
+    auto radix4 = [](double2 &v0, double2 &v1, double2 &v2, double2 &v3, double2 w1, double2 w2, double2 w3) {
         if (INV) { w1.y = -w1.y; w2.y = -w2.y; w3.y = -w3.y; }
         v1 = c_mul(v1, w1); v2 = c_mul(v2, w2); v3 = c_mul(v3, w3);
         dft4<INV>(v0, v1, v2, v3);
     };
-    {   // radix 4, Ns = 8 (both sequences, j = lane)
-        double2 a0 = r0[cc_ph(l)], a1 = r0[cc_ph(l + 32)], a2 = r0[cc_ph(l + 64)], a3 = r0[cc_ph(l + 96)];
-        double2 b0 = r1[cc_ph(l)], b1 = r1[cc_ph(l + 32)], b2 = r1[cc_ph(l + 64)], b3 = r1[cc_ph(l + 96)];
-        __syncwarp();
-        const int k = l & 7, ob = (l >> 3) * 32 + k;
+    double2 y[16];
+    {   // radix 4, Ns = 8: butterfly 8m + k reads positions k + 8(m + 4t), writes k + 8(4m + t)
         const double2 w1 = tws[CC_TW2 + k], w2 = tws[CC_TW2 + 8 + k], w3 = tws[CC_TW2 + 16 + k];
-        radix4(a0, a1, a2, a3, w1, w2, w3); radix4(b0, b1, b2, b3, w1, w2, w3);
-        r0[cc_ph(ob)] = a0; r0[cc_ph(ob + 8)] = a1; r0[cc_ph(ob + 16)] = a2; r0[cc_ph(ob + 24)] = a3;
-        r1[cc_ph(ob)] = b0; r1[cc_ph(ob + 8)] = b1; r1[cc_ph(ob + 16)] = b2; r1[cc_ph(ob + 24)] = b3;
-        __syncwarp();
+#pragma unroll
+        for (int m = 0; m < 4; m++) {
+            double2 v0 = x[m], v1 = x[m + 4], v2 = x[m + 8], v3 = x[m + 12];
+            radix4(v0, v1, v2, v3, w1, w2, w3);
+            y[4 * m] = v0; y[4 * m + 1] = v1; y[4 * m + 2] = v2; y[4 * m + 3] = v3;
+        }
     }
-    {   // radix 4, Ns = 32
-        double2 a0 = r0[cc_ph(l)], a1 = r0[cc_ph(l + 32)], a2 = r0[cc_ph(l + 64)], a3 = r0[cc_ph(l + 96)];
-        double2 b0 = r1[cc_ph(l)], b1 = r1[cc_ph(l + 32)], b2 = r1[cc_ph(l + 64)], b3 = r1[cc_ph(l + 96)];
-        __syncwarp();
-        const double2 w1 = tws[l], w2 = tws[CC_TW3 + l], w3 = tws[3 * l];
-        radix4(a0, a1, a2, a3, w1, w2, w3); radix4(b0, b1, b2, b3, w1, w2, w3);
-        last(w, l, a0); last(w, l + 32, a1); last(w, l + 64, a2); last(w, l + 96, a3);
-        last(w + 8, l, b0); last(w + 8, l + 32, b1); last(w + 8, l + 64, b2); last(w + 8, l + 96, b3);
-        __syncwarp();
+#pragma unroll
+    for (int u = 0; u < 4; u++) {   // radix 4, Ns = 32: butterfly l = k + 8u reads and writes positions k + 8(u + 4i)
+        const int l = k + 8 * u;
+        double2 v0 = y[u], v1 = y[u + 4], v2 = y[u + 8], v3 = y[u + 12];
+        radix4(v0, v1, v2, v3, tws[l], tws[CC_TW3 + l], tws[3 * l]);
+        x[u] = v0; x[u + 4] = v1; x[u + 8] = v2; x[u + 12] = v3;
     }
+}
+
+// the next transform's first pass from pass 3's registers: butterflies k and k + 8, stored in place as row[8j + t]
+template <bool INV>
+__device__ __forceinline__ void cc_pass1_store(const double2 (&x)[16], double2 *row, int k)
+{
+    double2 a[8], b[8];
+#pragma unroll
+    for (int t = 0; t < 8; t++) { a[t] = x[2 * t]; b[t] = x[2 * t + 1]; }
+    dft8<INV>(a);
+    dft8<INV>(b);
+    __syncwarp();                          // the sequence's other lanes have read their 16 values
+#pragma unroll
+    for (int t = 0; t < 8; t++) { row[cc_ph(8 * k + t)] = a[t]; row[cc_ph(8 * k + 64 + t)] = b[t]; }
+    __syncwarp();
 }
 
 __global__ void __launch_bounds__(CC_T, 2)
@@ -325,109 +338,148 @@ cfe_cluster_kernel(CfePlan pl, DemodParams p, int oldest)
     const int n_clusters = gridDim.x / CC_CL, cid = blockIdx.x / CC_CL;
     const int N = 16384, ring_len = p.bb_len;
     const double2 *__restrict__ twN = pl.tw;
-    if (threadIdx.x < 128) tws[threadIdx.x] = twN[threadIdx.x * (N / 128)];
-    else if (threadIdx.x < 128 + 24) { const int e = threadIdx.x - 128, m = e >> 3, k = e & 7; tws[CC_TW2 + e] = twN[(4 * (m + 1) * k) * (N / 128)]; }
-    else if (threadIdx.x < 128 + 24 + 32) { const int l = threadIdx.x - 152; tws[CC_TW3 + l] = twN[(2 * l) * (N / 128)]; }
+    for (int t = threadIdx.x; t < 128 + 24 + 32; t += CC_T) {
+        if (t < 128) tws[t] = twN[t * (N / 128)];
+        else if (t < 128 + 24) { const int e = t - 128, m = e >> 3, k = e & 7; tws[CC_TW2 + e] = twN[(4 * (m + 1) * k) * (N / 128)]; }
+        else { const int l = t - 152; tws[CC_TW3 + l] = twN[(2 * l) * (N / 128)]; }
+    }
     // The four-step twiddles W_N^(c*k1) are read from the same table the reference-order transforms use (a product of two
     // smaller tables breaks the exact conjugate symmetry of the table and with it the estimator's tie-breaks on symmetric
     // spectra). Their indices do not depend on the data, so the loads are issued ahead of the cluster barrier they follow.
     __syncthreads();
-    // peers' buffers
-    const double2 *rA[CC_CL], *rB[CC_CL];
-#pragma unroll
-    for (int s = 0; s < CC_CL; s++) { rA[s] = cluster.map_shared_rank(bufA, s); rB[s] = cluster.map_shared_rank(bufB, s); }
     bool arrived = false;
     cluster.sync();                        // every CTA of the cluster is resident before the first remote access
+    const int f = threadIdx.x >> 3, k = threadIdx.x & 7;                    // lane k of sequence f in the passes after the first
+    double2 *const rowA = bufA + f * CC_RS, *const rowB = bufB + f * CC_RS;
     for (int ch = cid; ch < p.n_channels; ch += n_clusters) {
+        double2 x[16];
         // ---- this CTA's 16 columns of the linearised ring (oqpskdemodulator.cpp:418-424) -> A[cc][r]: 256 B runs per r
-        double2 colv[8];
+        double2 colv[2][8];
         {
             const double2 *ring = p.bb + (size_t)ch * ring_len;
             const int cc = threadIdx.x & 15, r0i = threadIdx.x >> 4;
 #pragma unroll
-            for (int i = 0; i < 8; i++) {
-                int n = oldest + 128 * (r0i + 16 * i) + 16 * q + cc;
-                if (n >= ring_len) n -= ring_len;
-                if (n >= ring_len) n -= ring_len;
-                colv[i] = ring[n];
-            }
+            for (int h = 0; h < 2; h++)
+#pragma unroll
+                for (int i = 0; i < 8; i++) {
+                    int n = oldest + 128 * (r0i + 8 * h + 16 * i) + 16 * q + cc;
+                    if (n >= ring_len) n -= ring_len;
+                    if (n >= ring_len) n -= ring_len;
+                    colv[h][i] = ring[n];
+                }
         }
         // ---- P1: column FFT over r                                                   A[cc][k1]
-        // this thread's eight samples r = r0i + 16 i of column cc are butterfly r0i of the first pass: it runs from registers
-        dft8<false>(colv);
+        // this thread's samples r = r0i + 8h + 16 i of column cc are butterflies r0i and r0i + 8 of the first pass
+        dft8<false>(colv[0]);
+        dft8<false>(colv[1]);
         if (arrived) { cluster.barrier_wait(); arrived = false; }   // the peers have pulled the previous channel's P3 result out of A
         {
             const int cc = threadIdx.x & 15, r0i = threadIdx.x >> 4;
 #pragma unroll
-            for (int i = 0; i < 8; i++) bufA[cc * CC_RS + cc_ph(8 * r0i + i)] = colv[i];
+            for (int h = 0; h < 2; h++)
+#pragma unroll
+                for (int i = 0; i < 8; i++) bufA[cc * CC_RS + cc_ph(8 * (r0i + 8 * h) + i)] = colv[h][i];
         }
         __syncthreads();
-        cc_fft<false, false>(bufA, tws, [&](int f, int e, double2 v) { bufA[f * CC_RS + cc_ph(e)] = v; });
-        double2 tw8[8];
+        cc_load16(rowA, k, x);
+        cc_pass23<false>(x, k, tws);
+        cc_store16(rowA, k, x);
+        double2 tw8[2][8];
         {
             const int kk = threadIdx.x & 15, cc = threadIdx.x >> 4;
 #pragma unroll
-            for (int s = 0; s < 8; s++) tw8[s] = __ldg(&twN[((16 * s + cc) * (16 * q + kk)) & (N - 1)]);
+            for (int h = 0; h < 2; h++)
+#pragma unroll
+                for (int s = 0; s < 8; s++) tw8[h][s] = __ldg(&twN[((16 * s + cc + 8 * h) * (16 * q + kk)) & (N - 1)]);
         }
         cluster.sync();
         // rows k1 = 16q+kk, all c: B[kk][c] = A_src[cc][k1] * W_N^{c k1}   (kk fastest: contiguous remote reads)
         {
-            const int kk = threadIdx.x & 15, cc = threadIdx.x >> 4;
-            double2 x[8];
+            const int kk = threadIdx.x & 15;
 #pragma unroll
-            for (int s = 0; s < 8; s++) x[s] = c_mul(rA[s][cc * CC_RS + cc_ph(16 * q + kk)], tw8[s]);
-            dft8<false>(x);                // c = cc + 16 s: butterfly cc of row kk's first pass
+            for (int h = 0; h < 2; h++) {
+                const int cc = (threadIdx.x >> 4) + 8 * h;
+                double2 v[8];
 #pragma unroll
-            for (int s = 0; s < 8; s++) bufB[kk * CC_RS + cc_ph(8 * cc + s)] = x[s];
+                for (int s = 0; s < 8; s++) v[s] = c_mul(cluster.map_shared_rank(bufA, s)[cc * CC_RS + cc_ph(16 * q + kk)], tw8[h][s]);
+                dft8<false>(v);            // c = cc + 16 s: butterfly cc of row kk's first pass
+#pragma unroll
+                for (int s = 0; s < 8; s++) bufB[kk * CC_RS + cc_ph(8 * cc + s)] = v[s];
+            }
         }
         __syncthreads();
         // ---- P2: row FFT over c -> mask (:99-100) -> row IFFT, in place               B[kk][c]
-        cc_fft<false, false>(bufB, tws, [&](int f, int e, double2 v) {
-            const int k = (16 * q + f) + 128 * e;          // X[k1 + n1*k2]
-            if (!pl.is8400) { if (k >= pl.startbin && k <= pl.stopbin) v = make_double2(0.0, 0.0); }
-            else { const double w = pl.window[k]; v = make_double2(v.x * w, v.y * w); }
-            bufB[f * CC_RS + cc_ph(e)] = v;
-        });
-        cc_fft<true, true>(bufB, tws, [&](int f, int e, double2 v) { bufB[f * CC_RS + cc_ph(e)] = v; });
+        cc_load16(rowB, k, x);
+        cc_pass23<false>(x, k, tws);
+#pragma unroll
+        for (int e = 0; e < 16; e++) {
+            const int bin = (16 * q + f) + 128 * (k + 8 * e);  // X[k1 + n1*k2]
+            if (!pl.is8400) { if (bin >= pl.startbin && bin <= pl.stopbin) x[e] = make_double2(0.0, 0.0); }
+            else {
+                // the product is rounded on its own (it must not be contracted into the inverse butterflies' adds)
+                const double w = pl.window[bin];
+                x[e] = make_double2(__dmul_rn(x[e].x, w), __dmul_rn(x[e].y, w));
+            }
+        }
+        cc_pass1_store<true>(x, rowB, k);
+        cc_load16(rowB, k, x);
+        cc_pass23<true>(x, k, tws);
+        cc_store16(rowB, k, x);
         {
             const int cc = threadIdx.x & 15, kk = threadIdx.x >> 4;
 #pragma unroll
-            for (int s = 0; s < 8; s++) tw8[s] = __ldg(&twN[((16 * q + cc) * (16 * s + kk)) & (N - 1)]);
+            for (int h = 0; h < 2; h++)
+#pragma unroll
+                for (int s = 0; s < 8; s++) tw8[h][s] = __ldg(&twN[((16 * q + cc) * (16 * s + kk + 8 * h)) & (N - 1)]);
         }
         cluster.sync();                    // every peer has finished reading A (it passed the pull above before its own P2)
         // columns c = 16q+cc, all k1: A[cc][k1] = B_src[kk][c] * conj(W_N^{c k1})   (cc fastest: contiguous remote reads)
         {
-            const int cc = threadIdx.x & 15, kk = threadIdx.x >> 4;
-            double2 x[8];
+            const int cc = threadIdx.x & 15;
 #pragma unroll
-            for (int s = 0; s < 8; s++) {
-                double2 w = tw8[s]; w.y = -w.y;
-                x[s] = c_mul(rB[s][kk * CC_RS + cc_ph(16 * q + cc)], w);
+            for (int h = 0; h < 2; h++) {
+                const int kk = (threadIdx.x >> 4) + 8 * h;
+                double2 v[8];
+#pragma unroll
+                for (int s = 0; s < 8; s++) {
+                    double2 w = tw8[h][s]; w.y = -w.y;
+                    v[s] = c_mul(cluster.map_shared_rank(bufB, s)[kk * CC_RS + cc_ph(16 * q + cc)], w);
+                }
+                dft8<true>(v);             // k1 = kk + 16 s: butterfly kk of column cc's first pass
+#pragma unroll
+                for (int s = 0; s < 8; s++) bufA[cc * CC_RS + cc_ph(8 * kk + s)] = v[s];
             }
-            dft8<true>(x);                 // k1 = kk + 16 s: butterfly kk of column cc's first pass
-#pragma unroll
-            for (int s = 0; s < 8; s++) bufA[cc * CC_RS + cc_ph(8 * kk + s)] = x[s];
         }
         __syncthreads();
         // ---- P3: column IFFT over k1 -> square (:103) -> column FFT over r, in place  A[cc][k1]
-        cc_fft<true, false>(bufA, tws, [&](int f, int e, double2 v) {
-            bufA[f * CC_RS + cc_ph(e)] = make_double2(v.x * v.x - v.y * v.y, v.x * v.y + v.y * v.x);
-        });
-        cc_fft<false, true>(bufA, tws, [&](int f, int e, double2 v) { bufA[f * CC_RS + cc_ph(e)] = v; });
+        cc_load16(rowA, k, x);
+        cc_pass23<true>(x, k, tws);
+#pragma unroll
+        for (int e = 0; e < 16; e++) x[e] = make_double2(x[e].x * x[e].x - x[e].y * x[e].y, x[e].x * x[e].y + x[e].y * x[e].x);
+        cc_pass1_store<false>(x, rowA, k);
+        cc_load16(rowA, k, x);
+        cc_pass23<false>(x, k, tws);
+        cc_store16(rowA, k, x);
         {
             const int kk = threadIdx.x & 15, cc = threadIdx.x >> 4;
 #pragma unroll
-            for (int s = 0; s < 8; s++) tw8[s] = __ldg(&twN[((16 * s + cc) * (16 * q + kk)) & (N - 1)]);
+            for (int h = 0; h < 2; h++)
+#pragma unroll
+                for (int s = 0; s < 8; s++) tw8[h][s] = __ldg(&twN[((16 * s + cc + 8 * h) * (16 * q + kk)) & (N - 1)]);
         }
         cluster.sync();
         {
-            const int kk = threadIdx.x & 15, cc = threadIdx.x >> 4;
-            double2 x[8];
+            const int kk = threadIdx.x & 15;
 #pragma unroll
-            for (int s = 0; s < 8; s++) x[s] = c_mul(rA[s][cc * CC_RS + cc_ph(16 * q + kk)], tw8[s]);
-            dft8<false>(x);
+            for (int h = 0; h < 2; h++) {
+                const int cc = (threadIdx.x >> 4) + 8 * h;
+                double2 v[8];
 #pragma unroll
-            for (int s = 0; s < 8; s++) bufB[kk * CC_RS + cc_ph(8 * cc + s)] = x[s];
+                for (int s = 0; s < 8; s++) v[s] = c_mul(cluster.map_shared_rank(bufA, s)[cc * CC_RS + cc_ph(16 * q + kk)], tw8[h][s]);
+                dft8<false>(v);
+#pragma unroll
+                for (int s = 0; s < 8; s++) bufB[kk * CC_RS + cc_ph(8 * cc + s)] = v[s];
+            }
         }
         cluster.barrier_arrive();          // split barrier: this CTA is done reading its peers' A (waited on before A is refilled)
         arrived = true;
@@ -436,26 +488,24 @@ cfe_cluster_kernel(CfePlan pl, DemodParams p, int oldest)
         {
             double *y = pl.y + (size_t)ch * N;
             const bool bigchange = p.I[(size_t)I_ZERO_BB * p.cpad + ch] != 0;     // y[i]=20 pending (coarsefreqestimate.cpp:87)
-            const int kk = threadIdx.x & 15, k2b = threadIdx.x >> 4;
             // y is only ever read by the fold search, for bins within [lo-epb-1, hi+epb+1] (coarsefreqestimate.cpp:112-130):
-            // bins outside that window are neither loaded, evaluated (log10) nor stored
+            // bins outside that window are neither loaded, evaluated (log10) nor stored. Y[k1 + n1*k2] with k1 = 16q + f and
+            // k2 = k + 8e; fftshift (:105): i = k1 + n1*((k2 + n2/2) % n2). The four sequences of a warp fill 32-byte sectors.
             const int need_lo = pl.lo - pl.expectedpeakbin - 1, need_hi = pl.hi + pl.expectedpeakbin + 1;
-            double yo[8];                                                         // requested before the transform, consumed after it
+            double yo[16];                                                        // requested before the transform, consumed after it
 #pragma unroll
-            for (int i = 0; i < 8; i++) {
-                const int i_sh = (16 * q + kk) + 128 * ((k2b + 16 * i + 64) & 127);
-                yo[i] = (bigchange || i_sh < need_lo || i_sh > need_hi) ? 20.0 : y[i_sh];
+            for (int e = 0; e < 16; e++) {
+                const int i_sh = (16 * q + f) + 128 * ((k + 8 * e + 64) & 127);
+                yo[e] = (bigchange || i_sh < need_lo || i_sh > need_hi) ? 20.0 : y[i_sh];
             }
-            cc_fft<false, false>(bufB, tws, [&](int f, int e, double2 v) { bufB[f * CC_RS + cc_ph(e)] = v; });
-            __syncthreads();
+            cc_load16(rowB, k, x);
+            cc_pass23<false>(x, k, tws);
 #pragma unroll
-            for (int i = 0; i < 8; i++) {
-                const int k2 = k2b + 16 * i;
-                const int i_sh = (16 * q + kk) + 128 * ((k2 + 64) & 127);         // fftshift (:105)
+            for (int e = 0; e < 16; e++) {
+                const int i_sh = (16 * q + f) + 128 * ((k + 8 * e + 64) & 127);
                 if (i_sh < need_lo || i_sh > need_hi) continue;
-                const double2 x = bufB[kk * CC_RS + cc_ph(k2)];
                 // 10*log10(max(|x|,1)) = 5*log10(max(|x|^2,1))
-                y[i_sh] = yo[i] * 0.9 + 0.1 * 5 * log10_ge1(fmax(x.x * x.x + x.y * x.y, 1.0));   // :108
+                y[i_sh] = yo[e] * 0.9 + 0.1 * 5 * log10_ge1(fmax(x[e].x * x[e].x + x[e].y * x[e].y, 1.0));   // :108
             }
         }
         __syncthreads();
