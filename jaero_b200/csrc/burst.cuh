@@ -5,8 +5,12 @@
 
 namespace jb {
 
-static const int BURST_MAXEV = 8;          // trident-buffer fills that may complete within one internal chunk
-static const int BURST_CHUNK = 16384;      // internal chunk length (samples); fills complete >= 2*pdet.length apart
+// A peak restarts the trident buffer, so a fill completes tri_sz samples after the last peak and the next one at least tri_sz + 1
+// samples later: one internal chunk completes at most (BURST_CHUNK - 1) / (tri_sz + 1) + 1 fills (burst OQPSK, tri_sz 2633: 7;
+// MSK 1200, 8000: 3; MSK 600, 17920: 1). Each needs its own slot until the trident FFTs have run, and so does the fill still in
+// progress at the chunk's end; burst_create refuses a mode whose bound does not fit.
+static const int BURST_MAXEV = 8;          // trident-buffer slots per channel (fills completing within one internal chunk + 1)
+static const int BURST_CHUNK = 16384;      // internal chunk length (samples)
 static const int TRI_N = 32768;            // FFTr size (burstmskdemodulator.cpp:217)
 
 struct HilbertStream {                     // QJHilbertFilter (DSP.cpp:754-794) as a streaming FFT convolution

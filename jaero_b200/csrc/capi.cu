@@ -1594,6 +1594,7 @@ static int burst_create(const jaero_settings *s, int n_channels, int device, int
         p.ee = 0.015; btdiff_fd = SPS * 150;
     }
     if (kind == 0) { p.tri_nb = (int)rint(p.size_base * SPS); p.tri_nt = (int)rint(p.size_top * SPS); }
+    if ((BURST_CHUNK - 1) / (p.tri_sz + 1) + 2 > BURST_MAXEV) { set_error("burst: more trident fills per chunk than buffer slots"); return JAERO_E_ARG; }
     p.startstopstart = kind == 1 ? (int)(SPS * (1050)) : (int)(SPS * 500);
     p.btd1_len = (int)std::ceil(1.0 * SPS) + 1;
     int kk;

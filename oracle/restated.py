@@ -31,6 +31,7 @@ def lib():
         L.jor_burst_oqpsk_new.restype = vp; L.jor_burst_oqpsk_new.argtypes = [d, d, d, d, d]
         L.jor_aux_take.restype = l; L.jor_aux_take.argtypes = [vp, i, vp, l]
         L.jor_write.argtypes = [vp, vp, l]; L.jor_set_dcd.argtypes = [vp, i]
+        L.jor_burst_set_sql.argtypes = [vp, i]
         L.jor_soft_count.restype = l; L.jor_soft_count.argtypes = [vp]
         L.jor_soft_take.restype = l; L.jor_soft_take.argtypes = [vp, vp, l]
         L.jor_cfe_log_take.restype = l; L.jor_cfe_log_take.argtypes = [vp, vp, l, i]
@@ -69,6 +70,7 @@ class OracleDemod:
             self.h = lib().jor_burst_msk_new(fb, Fs, freq_center, lockingbw, signalthreshold)
         elif kind == "burst_oqpsk":
             self.h = lib().jor_burst_oqpsk_new(fb, Fs, freq_center, lockingbw, signalthreshold)
+            lib().jor_burst_set_sql(self.h, int(sql))
         else:
             self.h = lib().jor_demod_new(0 if kind == "oqpsk" else 1, fb, Fs, freq_center, lockingbw, fft_power,
                                          signalthreshold, int(afc), int(sql), int(cpureduce))
@@ -95,6 +97,8 @@ class OracleDemod:
         return out[:n].copy()
 
     def take_aux(self, which):
+        """burst kinds: 0 = EbNo of each burst, 1 = trident log (5 values per test), 2 = stream index of the input sample at which
+        each trident test ran (the sample that completed the fill). Each log is drained independently."""
         out = np.zeros(1 << 14, dtype=np.float64)
         n = lib().jor_aux_take(self.h, which, _p(out), len(out))
         return out[:n].copy()
@@ -284,12 +288,17 @@ class OracleCChannel:
 
 
 def run_demod_job(args):
-    """(kind, kw, pcm, chunk) -> (soft, state, aux0): one restated demodulator over one stream. Module-level so that tests can
-    farm channels out to a multiprocessing pool."""
+    """(kind, kw, pcm, chunk) -> (soft, state, aux0): one restated demodulator over one stream, written in pieces of `chunk`
+    samples, or of the successive lengths in `chunk` when it is a sequence. Module-level so that tests can farm channels out to a
+    multiprocessing pool."""
     kind, kw, pcm, chunk = args
     d = OracleDemod(kind, **kw)
-    for a in range(0, len(pcm), chunk):
-        d.write(pcm[a:a + chunk])
+    if np.ndim(chunk) == 0:
+        chunk = [chunk] * -(-len(pcm) // chunk)
+    a = 0
+    for n in chunk:
+        d.write(pcm[a:a + n]); a += n
+    assert a >= len(pcm)
     soft, st = d.take_soft(), d.state()
     aux = d.take_aux(0) if kind.startswith("burst") else np.zeros(0)
     d.close()

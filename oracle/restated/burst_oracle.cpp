@@ -78,6 +78,7 @@ BurstMskOracle::BurstMskOracle(double fb_, double Fs_, double fc_, double lbw_, 
     st_osc.SetFreq(fb / 2.0, (int)Fs); st_osc_half.SetFreq(fb / 2.0, (int)Fs);
     delayedsmpl.setLength(sps);
     n_sig_true = n_sig_false = 0;
+    nsamp = 0;
 }
 
 void BurstMskOracle::CenterFreqChangedSlot(double f)
@@ -148,6 +149,7 @@ void BurstMskOracle::writeData(const int16_t *ptr, long numofsamples)
             int distfrompeak = std::abs(maxtoppos - minvalbin);
             bool accept = minval > 500.0 && std::abs(distfrompeak - peakspacingbins) < std::abs(peakspacingbins / 20) && !(dcd) && !(cntr > 0 && cntr < (500 * SamplesPerSymbol));
             trident_log.push_back(minvalbin); trident_log.push_back(minval); trident_log.push_back(maxtoppos); trident_log.push_back(maxtopposhigh); trident_log.push_back(accept ? 1.0 : 0.0);
+            fill_log.push_back((double)(nsamp + i));
             if (accept) {
                 vol_gain = 1.4142 * (500.0 / (minval / 3));
                 double carrierphase = std::arg(out_base[minvalbin]) - (M_PI / 4.0);
@@ -234,6 +236,7 @@ void BurstMskOracle::writeData(const int16_t *ptr, long numofsamples)
             st_osc.WTnextFrame(); st_osc_half.WTnextFrame(); mixer2.WTnextFrame(); mixer_center.WTnextFrame();   // :744-748
         }
     }
+    nsamp += numofsamples;
 }
 } // namespace jor
 
@@ -281,6 +284,7 @@ BurstOqpskOracle::BurstOqpskOracle(double fb_, double Fs_, double fc_, double lb
     pt_d = 0; yui = 0; sig2_last = 0; symboltone_rotator = 1; startstop = -1; vol_gain = 1; cntr = 0;
     rotator_freq = 0;
     n_sig_true = n_sig_false = 0;
+    nsamp = 0;
 }
 
 void BurstOqpskOracle::writeData(const int16_t *ptr, long numofsamples)
@@ -331,6 +335,7 @@ void BurstOqpskOracle::writeData(const int16_t *ptr, long numofsamples)
             for (int k = 0; k < N / 2; k++) if ((std::abs(out_base[k])) > minval) { minval = std::abs(out_base[k]); minvalbin = k; }
             bool accept = (maxval > 500.0) && (fabs((((double)(maxvalbin - minvalbin))) * hzperbin) < 20.0);
             trident_log.push_back(minvalbin); trident_log.push_back(minval); trident_log.push_back(maxvalbin); trident_log.push_back(maxval); trident_log.push_back(accept ? 1.0 : 0.0);
+            fill_log.push_back((double)(nsamp + i));
             if (accept) {
                 double carrierphase = std::arg(out_base[(int)minvalbin]) - (M_PI / 4.0);
                 mixer2.SetFreq(hzperbin * minvalbin);
@@ -438,5 +443,6 @@ void BurstOqpskOracle::writeData(const int16_t *ptr, long numofsamples)
         sig2_last = sig2;                                                                          // :727
         mixer2.WTnextFrame(); st_osc.WTnextFrame(); st_osc_ref.WTnextFrame(); st_osc_quarter.WTnextFrame();
     }
+    nsamp += numofsamples;
 }
 } // namespace jor

@@ -23,15 +23,19 @@ void *jor_burst_oqpsk_new(double fb, double Fs, double freq_center, double locki
 { OrHandle *h = new OrHandle(); h->kind = 3; h->oq = 0; h->msk = 0; h->bmsk = 0; h->boq = new BurstOqpskOracle(fb, Fs, freq_center, lockingbw, signalthreshold); return h; }
 void jor_write(void *hv, const int16_t *pcm, long n)
 { OrHandle *h = (OrHandle *)hv; if (h->kind == 0) h->oq->writeData(pcm, n); else if (h->kind == 1) h->msk->writeData(pcm, n); else if (h->kind == 2) h->bmsk->writeData(pcm, n); else h->boq->writeData(pcm, n); }
+void jor_burst_set_sql(void *hv, int sql)          // burst OQPSK squelch (burstoqpskdemodulator.cpp setSQL)
+{ OrHandle *h = (OrHandle *)hv; if (h->kind == 3) h->boq->sql = (sql != 0); }
 void jor_set_dcd(void *hv, int d)
 { OrHandle *h = (OrHandle *)hv; if (h->kind == 0) h->oq->DCDstatSlot(d != 0); else if (h->kind == 1) h->msk->DCDstatSlot(d != 0); else if (h->kind == 2) h->bmsk->dcd = (d != 0); }
 static std::vector<short> &soft_of(OrHandle *h) { return h->kind == 0 ? h->oq->soft_out : (h->kind == 1 ? h->msk->soft_out : (h->kind == 2 ? h->bmsk->soft_out : h->boq->soft_out)); }
 long jor_soft_count(void *hv)
 { OrHandle *h = (OrHandle *)hv; return (long)soft_of(h).size(); }
-long jor_aux_take(void *hv, int which, double *out, long cap)     // burst: 0 = EbNo per burst, 1 = trident log (5 values per test)
+// burst: 0 = EbNo per burst, 1 = trident log (5 values per test), 2 = stream index of the sample that completed each fill
+long jor_aux_take(void *hv, int which, double *out, long cap)
 {
-    OrHandle *h = (OrHandle *)hv; if (h->kind < 2) return 0;
-    std::vector<double> &v = h->kind == 2 ? (which == 0 ? h->bmsk->ebno_log : h->bmsk->trident_log) : (which == 0 ? h->boq->ebno_log : h->boq->trident_log);
+    OrHandle *h = (OrHandle *)hv; if (h->kind < 2 || which < 0 || which > 2) return 0;
+    std::vector<double> &v = h->kind == 2 ? (which == 0 ? h->bmsk->ebno_log : which == 1 ? h->bmsk->trident_log : h->bmsk->fill_log)
+                                          : (which == 0 ? h->boq->ebno_log : which == 1 ? h->boq->trident_log : h->boq->fill_log);
     long n = (long)v.size(); if (n > cap) n = cap;
     memcpy(out, v.data(), n * sizeof(double)); v.erase(v.begin(), v.begin() + n); return n;
 }
