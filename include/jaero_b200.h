@@ -320,7 +320,18 @@ int jaero_ingest_flush(jaero_ingest *g, jaero_batch *b, size_t n_samples);
  * when input j * D1 arrives and an output m the audio frequency in force when input m * decimation arrives.
  * Filters (jaero_ddc_plan): real low-pass stages, h1 decimating by D1 and h2 by D2 (D1 * D2 = decimation; D2 = 1, h2 = {1} is a
  * single stage), whose composite response passes |f| <= bandwidth/2 around the offset within +-0.1 dB of its 0 Hz gain and
- * attenuates every tone with |f| >= bandwidth/2 + transition, up to +-input_rate/2 and aliases included, by at least 70 dB. */
+ * attenuates every tone with |f| >= bandwidth/2 + transition, up to +-input_rate/2 and aliases included, by at least 70 dB.
+ *
+ * Rational rates (jaero_ddc_plan_rational, jaero_ddc_create_rational): for a radio whose rate is not a multiple of 48 kHz, the
+ * output rate is Fs_out = input_rate * L / M for coprime L (interpolation, 1 to 256) and M (decimation). Stage 1 is as above with
+ * D1 dividing M; stage 2 is a polyphase resampler, M2 = M / D1:
+ *   w[i] = u[i / L] if L divides i, else 0   (u[j < 0] = 0);   v[m] = sum_k h2[k] w[m M2 - k]   (h2 sums to L: unit passband gain)
+ * and pcm[m] as above, with Fs_out = input_rate * L / M in S_c. Output m exists once input floor(m M / L) has arrived: N inputs
+ * give ceil(N L / M) outputs per channel, and everything output m reads has arrived by then. An output m uses the audio
+ * frequency in force when input floor(m M / L) arrives; the offset rule is unchanged. The output does not depend on how the
+ * stream is cut into writes. The filter specification is the one above, the images of the x L zero-stuffing included. With
+ * L = 1 every formula reduces to the one above term by term, and jaero_ddc_plan / jaero_ddc_create are exactly those calls.
+ * Every other jaero_ddc_* call works on either kind of handle. */
 #define JAERO_IQ_CU8 0   /* interleaved unsigned 8-bit I, Q */
 #define JAERO_IQ_CS16 1  /* interleaved signed 16-bit I, Q */
 typedef struct jaero_ddc jaero_ddc;
@@ -331,6 +342,13 @@ int jaero_ddc_plan(double input_rate, int decimation, double bandwidth, double t
  * [audio_hz - bandwidth/2, audio_hz + bandwidth/2] leaves (0, Fs_out/2). */
 int jaero_ddc_create(double input_rate, int decimation, int n_channels, const double *offset_hz, const double *audio_hz,
                      double bandwidth, double transition, double gain, int device_ordinal, jaero_ddc **out);
+/* The same at output rate input_rate * interpolation / decimation: stages = {L, D1, K1, M2, K2}, h2 the K2-tap prototype at
+ * L * input_rate / D1 (summing to L). Rejects L outside 1..256, a ratio with a common factor (reduce it), and a ratio for which no
+ * split meets the filter specification within the tap limits. */
+int jaero_ddc_plan_rational(double input_rate, int interpolation, int decimation, double bandwidth, double transition, int32_t stages[5],
+                            double *h1, double *h2);
+int jaero_ddc_create_rational(double input_rate, int interpolation, int decimation, int n_channels, const double *offset_hz,
+                              const double *audio_hz, double bandwidth, double transition, double gain, int device_ordinal, jaero_ddc **out);
 void jaero_ddc_destroy(jaero_ddc *d);
 /* n_iq complex samples, format JAERO_IQ_*. HOST iq (copied before the call returns) */
 int jaero_ddc_write(jaero_ddc *d, const void *iq, size_t n_iq, int format);

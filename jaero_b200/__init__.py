@@ -71,7 +71,7 @@ EXPORTS = ["jaero_last_error", "jaero_device_count", "jaero_batch_create", "jaer
            "jaero_reasm_push_r", "jaero_reasm_push_t_packet", "jaero_reasm_pending", "jaero_reasm_pop", "jaero_reasm_get_stats",
            "jaero_ddc_plan", "jaero_ddc_create", "jaero_ddc_destroy", "jaero_ddc_write", "jaero_ddc_write_device", "jaero_ddc_output",
            "jaero_ddc_read_pcm", "jaero_ddc_set_stream", "jaero_ddc_set_offset", "jaero_ddc_set_audio_freq", "jaero_ddc_get_stats",
-           "jaero_ddc_launch_count",
+           "jaero_ddc_launch_count", "jaero_ddc_plan_rational", "jaero_ddc_create_rational",
            "jaero_scan_create", "jaero_scan_destroy", "jaero_scan_write", "jaero_scan_write_device", "jaero_scan_set_stream",
            "jaero_scan_reset", "jaero_scan_read", "jaero_scan_launch_count", "jaero_scan_find_carriers"]
 MODES = {0: "unknown", 1: "msk600", 2: "msk1200", 3: "oqpsk8400", 4: "oqpsk10500"}
@@ -181,6 +181,8 @@ def lib():
         L.jaero_reasm_get_stats.argtypes = [vp, vp, vp, vp, vp]
         L.jaero_ddc_plan.argtypes = [d, i, d, d, vp, vp, vp]
         L.jaero_ddc_create.argtypes = [d, i, i, vp, vp, d, d, d, i, ctypes.POINTER(vp)]
+        L.jaero_ddc_plan_rational.argtypes = [d, i, i, d, d, vp, vp, vp]
+        L.jaero_ddc_create_rational.argtypes = [d, i, i, i, vp, vp, d, d, d, i, ctypes.POINTER(vp)]
         L.jaero_ddc_destroy.argtypes = [vp]; L.jaero_ddc_destroy.restype = None
         L.jaero_ddc_write.argtypes = [vp, vp, sz, i]; L.jaero_ddc_write_device.argtypes = [vp, vp, sz, i]
         L.jaero_ddc_output.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(sz), ctypes.POINTER(sz)]
@@ -786,31 +788,48 @@ class Reassembler:
             pass
 
 
-def ddc_plan(input_rate, decimation, bandwidth, transition):
-    """The down-converter's filter stages for a set-up (host only, no device): dict(D1, K1, D2, K2, h1, h2)."""
-    st = np.zeros(4, dtype=np.int32)
-    _check(lib().jaero_ddc_plan(float(input_rate), int(decimation), float(bandwidth), float(transition), _p(st), None, None))
-    h1 = np.zeros(int(st[1])); h2 = np.zeros(int(st[3]))
-    _check(lib().jaero_ddc_plan(float(input_rate), int(decimation), float(bandwidth), float(transition), _p(st), _p(h1), _p(h2)))
-    return dict(D1=int(st[0]), K1=int(st[1]), D2=int(st[2]), K2=int(st[3]), h1=h1, h2=h2)
+def ddc_plan(input_rate, decimation, bandwidth, transition, interpolation=1):
+    """The down-converter's filter stages for a set-up (host only, no device): dict(L, D1, K1, D2, K2, h1, h2), output rate
+    input_rate * L / (D1 * D2). h2 is the K2-tap stage-2 prototype at L * input_rate / D1, summing to L."""
+    st = np.zeros(5, dtype=np.int32)
+    args = (float(input_rate), int(interpolation), int(decimation), float(bandwidth), float(transition), _p(st))
+    _check(lib().jaero_ddc_plan_rational(*args, None, None))
+    h1 = np.zeros(int(st[2])); h2 = np.zeros(int(st[4]))
+    _check(lib().jaero_ddc_plan_rational(*args, _p(h1), _p(h2)))
+    return dict(L=int(st[0]), D1=int(st[1]), K1=int(st[2]), D2=int(st[3]), K2=int(st[4]), h1=h1, h2=h2)
+
+
+def rate_ratio(input_rate, output_rate=48000.0):
+    """(L, M), coprime, with output_rate = input_rate * L / M: the interpolation and decimation of a Ddc for a radio's rate.
+    Exact for whole-hertz rates; raises ValueError for any other rate or when L exceeds 256."""
+    from fractions import Fraction
+    for r in (input_rate, output_rate):
+        if not (float(r) > 0 and float(r) == int(float(r))):
+            raise ValueError("rate_ratio: rates must be positive whole hertz, got %r" % (r,))
+    q = Fraction(int(float(output_rate)), int(float(input_rate)))
+    if q.numerator > 256:
+        raise ValueError("rate_ratio: interpolation %d exceeds 256 (%s Hz -> %s Hz)" % (q.numerator, input_rate, output_rate))
+    return q.numerator, q.denominator
 
 
 class Ddc:
     """Wideband IQ digital down-converter (include/jaero_b200.h, jaero_ddc_*): one cu8 / cs16 IQ stream at input_rate ->
-    n_channels real int16 PCM streams at input_rate / decimation, channel c tuned to offsets_hz[c] and placed at audio_hz[c]."""
+    n_channels real int16 PCM streams at output_rate = input_rate * interpolation / decimation, channel c tuned to offsets_hz[c]
+    and placed at audio_hz[c]. rate_ratio gives (interpolation, decimation) for a radio's rate."""
     FORMATS = {"cu8": IQ_CU8, "cs16": IQ_CS16, IQ_CU8: IQ_CU8, IQ_CS16: IQ_CS16}
 
-    def __init__(self, input_rate, decimation, offsets_hz, audio_hz, bandwidth, transition, gain=1.0, device=0):
+    def __init__(self, input_rate, decimation, offsets_hz, audio_hz, bandwidth, transition, gain=1.0, device=0, interpolation=1):
         off = np.ascontiguousarray(offsets_hz, dtype=np.float64).reshape(-1)
         if len(off) == 0:
             raise JaeroError("at least one channel is needed")
         aud = np.ascontiguousarray(np.broadcast_to(np.asarray(audio_hz, dtype=np.float64), off.shape))
         self.n = len(off)
-        self.input_rate, self.decimation = float(input_rate), int(decimation)
+        self.input_rate, self.decimation, self.interpolation = float(input_rate), int(decimation), int(interpolation)
+        self.output_rate = self.input_rate * self.interpolation / self.decimation
         self.h = ctypes.c_void_p()
-        _check(lib().jaero_ddc_create(self.input_rate, self.decimation, self.n, _p(off), _p(aud), float(bandwidth), float(transition),
-                                      float(gain), device, ctypes.byref(self.h)))
-        self.plan = ddc_plan(input_rate, decimation, bandwidth, transition)
+        _check(lib().jaero_ddc_create_rational(self.input_rate, self.interpolation, self.decimation, self.n, _p(off), _p(aud),
+                                               float(bandwidth), float(transition), float(gain), device, ctypes.byref(self.h)))
+        self.plan = ddc_plan(input_rate, decimation, bandwidth, transition, interpolation)
 
     @staticmethod
     def _iq(iq, fmt):
@@ -959,8 +978,9 @@ CHANNEL_SETTINGS = {
 }
 
 
-def channel_plan(carriers, input_rate, decimation):
-    """Groups find_carriers' detections by mode into down-converter and demodulator arguments.
+def channel_plan(carriers, input_rate, decimation, interpolation=1):
+    """Groups find_carriers' detections by mode into down-converter and demodulator arguments, for a Ddc at output rate
+    input_rate * interpolation / decimation (rate_ratio gives the pair).
 
     -> (plans, unplanned). plans[mode] = dict(ddc=kwargs of Ddc, demod=kwargs of DemodBatch, carriers=the group's detections), one
     per continuous mode found, channels in ascending frequency. The gain puts the group's strongest carrier at 0.2 sqrt(2) rms of
@@ -977,8 +997,9 @@ def channel_plan(carriers, input_rate, decimation):
         s = CHANNEL_SETTINGS[mode]
         gain = 0.2 * np.sqrt(2) / np.sqrt(max(c["power"] for c in group))
         out[mode] = dict(
-            ddc=dict(input_rate=float(input_rate), decimation=int(decimation), offsets_hz=[c["center_hz"] for c in group],
-                     audio_hz=s["audio_hz"], bandwidth=s["bandwidth"], transition=s["transition"], gain=float(gain)),
+            ddc=dict(input_rate=float(input_rate), decimation=int(decimation), interpolation=int(interpolation),
+                     offsets_hz=[c["center_hz"] for c in group], audio_hz=s["audio_hz"], bandwidth=s["bandwidth"],
+                     transition=s["transition"], gain=float(gain)),
             demod=dict(kind=s["kind"], n_channels=len(group), fb=s["fb"], freq_center=s["audio_hz"], lockingbw=s["lockingbw"]),
             carriers=group)
     return out, unplanned

@@ -19,6 +19,7 @@
 #include <cstdlib>
 #include <initializer_list>
 #include <new>
+#include <numeric>
 #include <vector>
 
 namespace jb {
@@ -2086,39 +2087,50 @@ static void kaiser_lowpass(double fs, double fpass, double fstop, int n, double 
     for (int k = 0; k < n; k++) h[k] /= sum;
 }
 
-struct DdcPlan { int D1, K1, D2, K2; double fs1; };
+static const int DDC_MAX_INTERPOLATION = 256;
 
-// The split D = D1 * D2 with the fewest multiply-adds per output (a stage-1 tap is a complex x complex product, twice a
-// stage-2 tap). Stage 1 passes B/2 and stops Fs1 - B/2 - transition, everything that would alias into stage 2's passband;
-// stage 2 passes B/2 and stops B/2 + transition.
-static int ddc_plan_stages(double fs, int D, double B, double dT, DdcPlan *out, const char *fn)
+struct DdcPlan { int L, D1, K1, D2, K2; double fs1; };
+
+// The split M = D1 * D2 with the fewest multiply-adds per output: 8 (D2 / L) K1 + 4 ceil(K2 / L) flop (a stage-1 tap is a
+// complex x complex product, twice a stage-2 tap, and of the K2 stage-2 taps only every L-th meets a sample that is not a
+// stuffed zero). The search compares that count times L / 4, an integer. Stage 1 passes B/2 and stops Fs1 - B/2 - transition,
+// everything that would alias into stage 2's passband; stage 2, at L * Fs1, passes B/2 and stops B/2 + transition, which also
+// removes the images of the x L zero-stuffing. For L = 1 a single stage (D2 = 1, h2 = {1}) is a candidate and a stage 1 that
+// does not decimate is not; for L > 1 stage 2 always interpolates, so every divisor D1 of M is a candidate.
+static int ddc_plan_stages(double fs, int L, int M, double B, double dT, DdcPlan *out, const char *fn)
 {
-    const double fs_out = fs / D, fp = 0.5 * B, fst = 0.5 * B + dT;
-    if (!(fs > 0) || D < 1 || !(B > 0) || !(dT > 0)) { set_error(std::string(fn) + ": rates, bandwidth and transition must be positive"); return JAERO_E_ARG; }
+    const double fs_out = fs * L / M, fp = 0.5 * B, fst = 0.5 * B + dT;
+    if (!(fs > 0) || M < 1 || !(B > 0) || !(dT > 0)) { set_error(std::string(fn) + ": rates, bandwidth and transition must be positive"); return JAERO_E_ARG; }
+    if (L < 1 || L > DDC_MAX_INTERPOLATION) { set_error(std::string(fn) + ": interpolation must be 1 to " + std::to_string(DDC_MAX_INTERPOLATION)); return JAERO_E_ARG; }
+    if (std::gcd(L, M) != 1) { set_error(std::string(fn) + ": interpolation and decimation have a common factor; reduce the ratio L/M"); return JAERO_E_ARG; }
     if (!(fst <= 0.5 * fs_out)) { set_error(std::string(fn) + ": bandwidth/2 + transition must not exceed half the output rate"); return JAERO_E_ARG; }
     long best = -1;
-    for (int D1 = 1; D1 <= D; D1++) {
-        if (D % D1) continue;
-        DdcPlan c{D1, 0, D / D1, 1, fs / D1};
-        if (c.D2 == 1) c.K1 = kaiser_length(fs, fp, fst);
+    for (int D1 = 1; D1 <= M; D1++) {
+        if (M % D1) continue;
+        DdcPlan c{L, D1, 0, M / D1, 1, fs / D1};
+        if (L == 1 && c.D2 == 1) c.K1 = kaiser_length(fs, fp, fst);
         else {
-            if (D1 == 1) continue;                                   // a stage 1 that does not decimate only adds work
+            if (L == 1 && D1 == 1) continue;                         // a stage 1 that does not decimate only adds work
+            if (!(c.fs1 - fst > fp)) continue;                       // stage 1's output rate leaves it no stopband
             c.K1 = kaiser_length(fs, fp, c.fs1 - fst);
-            c.K2 = kaiser_length(c.fs1, fp, fst);
+            c.K2 = kaiser_length(c.fs1 * L, fp, fst);
         }
         if (c.K1 > DDC_MAX_TAPS || c.K2 > DDC_MAX_TAPS || (DDC_TILE_J - 1) * D1 + c.K1 > DDC_MAX_TILE) continue;
-        const long cost = 2L * c.D2 * c.K1 + c.K2;
+        const long cost = 2L * c.D2 * c.K1 + (long)L * ((c.K2 + L - 1) / L);
         if (best < 0 || cost < best) { best = cost; *out = c; }
     }
     if (best < 0) { set_error(std::string(fn) + ": no two-stage split of this decimation meets the filter specification within the tap limits"); return JAERO_E_ARG; }
     return JAERO_OK;
 }
+// h2 sums to L: the zero-stuffing divides the signal's level by L, so the passband gain is 1.
 static void ddc_design(double fs, double B, double dT, const DdcPlan &c, double *h1, double *h2)
 {
     const double fp = 0.5 * B, fst = 0.5 * B + dT;
-    if (c.D2 == 1) { kaiser_lowpass(fs, fp, fst, c.K1, h1); h2[0] = 1.0; return; }
+    if (c.L == 1 && c.D2 == 1) { kaiser_lowpass(fs, fp, fst, c.K1, h1); h2[0] = 1.0; return; }
     kaiser_lowpass(fs, fp, c.fs1 - fst, c.K1, h1);
-    kaiser_lowpass(c.fs1, fp, fst, c.K2, h2);
+    kaiser_lowpass(c.fs1 * c.L, fp, fst, c.K2, h2);
+    if (c.L > 1)
+        for (int k = 0; k < c.K2; k++) h2[k] *= c.L;
 }
 // round(f / fs * 2^32) mod 2^32
 static uint32_t tuning_word(double f, double fs) { return (uint32_t)(uint64_t)llround(f / fs * 4294967296.0); }
@@ -2168,12 +2180,15 @@ static bool ddc_audio_ok(const jaero_ddc *d, double hz) { return std::isfinite(h
 
 extern "C" {
 
-int jaero_ddc_plan(double input_rate, int decimation, double bandwidth, double transition, int32_t stages[4], double *h1, double *h2)
+// jaero_ddc_plan and jaero_ddc_plan_rational: stages receives {D1, K1, D2, K2}, preceded by L when with_l
+static int ddc_plan_query(double input_rate, int L, int M, double bandwidth, double transition, int32_t *stages, bool with_l, double *h1,
+                          double *h2, const char *fn)
 {
-    if (!stages) { set_error("jaero_ddc_plan: null argument"); return JAERO_E_ARG; }
+    if (!stages) { set_error(std::string(fn) + ": null argument"); return JAERO_E_ARG; }
     DdcPlan c;
-    const int r = ddc_plan_stages(input_rate, decimation, bandwidth, transition, &c, "jaero_ddc_plan");
+    const int r = ddc_plan_stages(input_rate, L, M, bandwidth, transition, &c, fn);
     if (r) return r;
+    if (with_l) *stages++ = c.L;
     stages[0] = c.D1; stages[1] = c.K1; stages[2] = c.D2; stages[3] = c.K2;
     if (h1 && h2) ddc_design(input_rate, bandwidth, transition, c, h1, h2);
     else if (h1 || h2) {
@@ -2185,48 +2200,75 @@ int jaero_ddc_plan(double input_rate, int decimation, double bandwidth, double t
     return JAERO_OK;
 }
 
-int jaero_ddc_create(double input_rate, int decimation, int n_channels, const double *offset_hz, const double *audio_hz, double bandwidth,
-                     double transition, double gain, int device, jaero_ddc **out)
+static int ddc_create(double input_rate, int L, int M, int n_channels, const double *offset_hz, const double *audio_hz, double bandwidth,
+                      double transition, double gain, int device, jaero_ddc **out, const char *fn)
 {
-    if (!out || n_channels <= 0 || !offset_hz || !audio_hz || !std::isfinite(gain)) { set_error("jaero_ddc_create: bad argument"); return JAERO_E_ARG; }
+    const std::string f(fn);
+    if (!out || n_channels <= 0 || !offset_hz || !audio_hz || !std::isfinite(gain)) { set_error(f + ": bad argument"); return JAERO_E_ARG; }
     DdcPlan c;
-    { const int r = ddc_plan_stages(input_rate, decimation, bandwidth, transition, &c, "jaero_ddc_create"); if (r) return r; }
-    const double fs_out = input_rate / decimation;
+    { const int r = ddc_plan_stages(input_rate, L, M, bandwidth, transition, &c, fn); if (r) return r; }
+    const double fs_out = input_rate * L / M;
     for (int ch = 0; ch < n_channels; ch++) {
         if (!(std::isfinite(offset_hz[ch]) && fabs(offset_hz[ch]) <= 0.5 * input_rate - 0.5 * bandwidth)) {
-            set_error("jaero_ddc_create: channel " + std::to_string(ch) + ": |offset| must not exceed input_rate/2 - bandwidth/2"); return JAERO_E_ARG; }
+            set_error(f + ": channel " + std::to_string(ch) + ": |offset| must not exceed input_rate/2 - bandwidth/2"); return JAERO_E_ARG; }
         if (!(std::isfinite(audio_hz[ch]) && audio_hz[ch] - 0.5 * bandwidth > 0 && audio_hz[ch] + 0.5 * bandwidth < 0.5 * fs_out)) {
-            set_error("jaero_ddc_create: channel " + std::to_string(ch) + ": the audio passband must lie inside (0, output_rate/2)"); return JAERO_E_ARG; }
+            set_error(f + ": channel " + std::to_string(ch) + ": the audio passband must lie inside (0, output_rate/2)"); return JAERO_E_ARG; }
     }
     CreateGuard<jaero_ddc> guard(jaero_ddc_destroy);
-    { const int e = guard.begin("jaero_ddc_create", device); if (e) return e; }
+    { const int e = guard.begin(fn, device); if (e) return e; }
     jaero_ddc *d = guard.obj;
     d->own_stream = d->stream;
     d->fs_in = input_rate; d->fs_out = fs_out; d->B = bandwidth;
     DdcParams &p = d->p;
     p.n_channels = n_channels; p.cpad = (n_channels + 31) & ~31;
-    p.D1 = c.D1; p.K1 = c.K1; p.D2 = c.D2; p.K2 = c.K2;
+    p.L = c.L; p.D1 = c.D1; p.K1 = c.K1; p.D2 = c.D2; p.K2 = c.K2;
+    p.R = (c.K2 + c.L - 1) / c.L;
+    // the first output of a write reads back R - 1 rows from q >= j_lo - 1 (L > 1) or K2 - 1 rows from q >= j_lo (L = 1)
+    p.H2 = c.L == 1 ? c.K2 - 1 : p.R;
     p.scale = gain * 32768.0;
     d->h1.resize(c.K1);
     std::vector<double> h2(c.K2);
     ddc_design(input_rate, bandwidth, transition, c, d->h1.data(), h2.data());
+    std::vector<double> h2p((size_t)c.L * p.R, 0.0);                 // [L][R] per-phase taps, h2p[phi][r] = h2[phi + r L]
+    for (int k = 0; k < c.K2; k++) h2p[(size_t)(k % c.L) * p.R + k / c.L] = h2[k];
     d->T.resize(n_channels); d->S.resize(n_channels);
     for (int ch = 0; ch < n_channels; ch++) { d->T[ch] = tuning_word(offset_hz[ch], input_rate); d->S[ch] = tuning_word(audio_hz[ch], fs_out); }
     d->h1c.assign((size_t)c.K1 * p.cpad, make_double2(0.0, 0.0));
     const size_t cp = p.cpad;
     double2 *h1c; double *dh2; uint32_t *T, *S;
     int rc = 0;
-    rc |= owned_alloc(d, &h1c, (size_t)c.K1 * cp); rc |= owned_alloc(d, &dh2, (size_t)c.K2);
+    rc |= owned_alloc(d, &h1c, (size_t)c.K1 * cp); rc |= owned_alloc(d, &dh2, h2p.size());
     rc |= owned_alloc(d, &T, cp); rc |= owned_alloc(d, &S, cp);
-    rc |= owned_alloc(d, &p.xhist, (size_t)std::max(1, c.K1 - 1)); rc |= owned_alloc(d, &p.uhist, (size_t)std::max(1, c.K2 - 1) * cp);
+    rc |= owned_alloc(d, &p.xhist, (size_t)std::max(1, c.K1 - 1)); rc |= owned_alloc(d, &p.uhist, (size_t)std::max(1, p.H2) * cp);
     rc |= owned_alloc(d, &p.clipped, cp);
     if (rc) return JAERO_E_CUDA;
     p.h1c = h1c; p.h2 = dh2; p.T = T; p.S = S;
-    JB_CUDA(cudaMemcpyAsync(dh2, h2.data(), c.K2 * sizeof(double), cudaMemcpyHostToDevice, d->stream));
+    JB_CUDA(cudaMemcpyAsync(dh2, h2p.data(), h2p.size() * sizeof(double), cudaMemcpyHostToDevice, d->stream));
     if (ddc_upload_offset(d, -1) || ddc_upload_words(d, d->S, p.S, -1)) return JAERO_E_CUDA;
     JB_CUDA(cudaStreamSynchronize(d->stream));                       // the zeroed histories and the tables are in place
     *out = guard.release();
     return JAERO_OK;
+}
+
+int jaero_ddc_plan(double input_rate, int decimation, double bandwidth, double transition, int32_t stages[4], double *h1, double *h2)
+{
+    return ddc_plan_query(input_rate, 1, decimation, bandwidth, transition, stages, false, h1, h2, "jaero_ddc_plan");
+}
+int jaero_ddc_plan_rational(double input_rate, int interpolation, int decimation, double bandwidth, double transition, int32_t stages[5],
+                            double *h1, double *h2)
+{
+    return ddc_plan_query(input_rate, interpolation, decimation, bandwidth, transition, stages, true, h1, h2, "jaero_ddc_plan_rational");
+}
+int jaero_ddc_create(double input_rate, int decimation, int n_channels, const double *offset_hz, const double *audio_hz, double bandwidth,
+                     double transition, double gain, int device, jaero_ddc **out)
+{
+    return ddc_create(input_rate, 1, decimation, n_channels, offset_hz, audio_hz, bandwidth, transition, gain, device, out, "jaero_ddc_create");
+}
+int jaero_ddc_create_rational(double input_rate, int interpolation, int decimation, int n_channels, const double *offset_hz,
+                              const double *audio_hz, double bandwidth, double transition, double gain, int device, jaero_ddc **out)
+{
+    return ddc_create(input_rate, interpolation, decimation, n_channels, offset_hz, audio_hz, bandwidth, transition, gain, device, out,
+                      "jaero_ddc_create_rational");
 }
 void jaero_ddc_destroy(jaero_ddc *d)
 {
@@ -2246,12 +2288,13 @@ int jaero_ddc_write_device(jaero_ddc *d, const void *d_iq, size_t n, int format)
     JB_CUDA(cudaSetDevice(d->device));
     DdcParams &p = d->p;
     const long long n0 = d->n_in, D = (long long)p.D1 * p.D2;
-    const size_t M = (size_t)((n0 + (long long)n + D - 1) / D - (n0 + D - 1) / D);
+    // outputs m with floor(m D / L) in [n0, n0 + n): ceil((n0 + n) L / D) - ceil(n0 L / D)
+    const size_t M = (size_t)(((n0 + (long long)n) * p.L + D - 1) / D - (n0 * p.L + D - 1) / D);
     const size_t J = (size_t)((n0 + (long long)n + p.D1 - 1) / p.D1 - (n0 + p.D1 - 1) / p.D1);
     const size_t stride = std::max<size_t>(8, (M + 7) & ~(size_t)7);   // 16-byte rows: jaero_batch_write_device reads them in place
     if (n > 0) {
         // a failed write leaves the output of the previous one described
-        if (grow(&d->d_x, &d->x_cap, (size_t)(p.K1 - 1) + n, d->stream) || grow(&d->d_u, &d->u_cap, ((size_t)(p.K2 - 1) + J) * p.cpad, d->stream) ||
+        if (grow(&d->d_x, &d->x_cap, (size_t)(p.K1 - 1) + n, d->stream) || grow(&d->d_u, &d->u_cap, ((size_t)p.H2 + J) * p.cpad, d->stream) ||
             grow(&d->d_pcm, &d->pcm_cap, (size_t)p.n_channels * stride, d->stream)) return JAERO_E_CUDA;
         if (ddc_run(p, d_iq, format, n0, (long long)n, d->d_x, d->d_u, d->d_pcm, stride, d->stream, &d->launches)) return JAERO_E_CUDA;
         d->n_in += (long long)n;

@@ -271,18 +271,25 @@ def replica_offsets(r0, r1, span_hz=300.0, seed0=0xB0057):
 def wideband_iq(envelopes, offsets_hz, Fs_in, ebn0_db, fmt="cs16", seed=0, fb=10500.0, Fs=48000.0, rms=0.25, return_levels=False):
     """One software-radio IQ stream carrying several channels (the input of the down-converter, jaero_b200.Ddc).
 
-    envelopes: complex 48 kHz envelopes (oqpsk_envelope / msk_envelope outputs). Each is upsampled to Fs_in with
-    scipy.signal.resample_poly, shifted to its offset (Hz from the centre frequency) and given the power that puts it at
+    envelopes: complex 48 kHz envelopes (oqpsk_envelope / msk_envelope outputs). Each is resampled to Fs_in with
+    scipy.signal.resample_poly (up Fs_in / Fs for an integer multiple, otherwise the reduced ratio up / down of two whole-hertz
+    rates), shifted to its offset (Hz from the centre frequency) and given the power that puts it at
     ebn0_db (scalar or one per envelope) over complex white noise, for bit rate fb (scalar or one per envelope). The sum is
     scaled to `rms` of full scale and quantised to fmt: 'cu8' (uint8, v = round(128 x + 127.5)) or 'cs16' (int16,
     v = round(32768 x)), interleaved I, Q. With return_levels, also returns each envelope's rms in full-scale units."""
+    from fractions import Fraction
     from scipy.signal import resample_poly
     D = int(round(Fs_in / Fs))
-    assert abs(D * Fs - Fs_in) < 1e-6 * Fs_in, "Fs_in must be an integer multiple of Fs"
+    if abs(D * Fs - Fs_in) < 1e-6 * Fs_in:
+        up, down = D, 1
+    else:
+        assert float(Fs_in) == int(Fs_in) and float(Fs) == int(Fs), "Fs_in / Fs must be a ratio of whole-hertz rates"
+        q = Fraction(int(Fs_in), int(Fs))
+        up, down = q.numerator, q.denominator
     k = len(envelopes)
     ebn0 = np.broadcast_to(np.asarray(ebn0_db, dtype=np.float64), (k,))
     fbs = np.broadcast_to(np.asarray(fb, dtype=np.float64), (k,))
-    n = max(len(e) for e in envelopes) * D
+    n = -(-max(len(e) for e in envelopes) * up // down)
     rng = np.random.default_rng(seed)
     # N0 = 1: complex noise of variance Fs_in per sample; envelope i gets power (Eb/N0)_i * fb_i
     x = (rng.standard_normal(n) + 1j * rng.standard_normal(n)) * np.sqrt(Fs_in / 2.0)
@@ -291,11 +298,11 @@ def wideband_iq(envelopes, offsets_hz, Fs_in, ebn0_db, fmt="cs16", seed=0, fb=10
     for i, (e, f) in enumerate(zip(envelopes, offsets_hz)):
         e = np.asarray(e, dtype=np.complex128)
         amps[i] = np.sqrt(10 ** (ebn0[i] / 10.0) * fbs[i] / np.mean(np.abs(e) ** 2))
-        up = resample_poly(e, D, 1)
-        for a in range(0, len(up), step):
-            t = np.arange(a, min(a + step, len(up)))
-            x[t] += amps[i] * up[t] * np.exp(2j * np.pi * float(f) * t / Fs_in)
-        del up
+        y = resample_poly(e, up, down)
+        for a in range(0, len(y), step):
+            t = np.arange(a, min(a + step, len(y)))
+            x[t] += amps[i] * y[t] * np.exp(2j * np.pi * float(f) * t / Fs_in)
+        del y
     scale = rms / np.sqrt(np.mean(np.abs(x) ** 2))
     x *= scale
     iq = np.empty(2 * n)
