@@ -123,8 +123,8 @@ int jaero_batch_set_afc(jaero_batch *b, int state);
 int jaero_batch_set_sql(jaero_batch *b, int state);
 int jaero_batch_set_cpu_reduce(jaero_batch *b, int state);
 /* Seating of the channels inside the 10500 bps kernel. Channels never interact, so results do not depend on it; throughput does:
- * the library seats channels with the same symbol-timing phase next to each other (automatically, every JAERO_REGROUP_EPOCHS
- * estimator epochs; this call does it now when slot_of is NULL, or installs the given permutation slot_of[channel] = seat). */
+ * the library seats channels with the same symbol-timing phase next to each other (automatically, every 128 estimator epochs
+ * after the first two checks; this call does it now when slot_of is NULL, or installs the given permutation slot_of[channel] = seat). */
 int jaero_batch_regroup(jaero_batch *b, const int32_t *slot_of);
 /* connect(demodulator, SIGNAL(SignalStatus(bool)), aerol, SLOT(SignalStatusSlot(bool))) (JAERO/mainwindow.cpp:432,508): with it, a
  * SignalStatus(false) clears the channel's DCD in the kernel and is handed to the device frame layer (jaero_pchannel_process_batch /
@@ -144,7 +144,7 @@ int jaero_batch_set_stream(jaero_batch *b, void *cuda_stream);
 int jaero_batch_set_profiling(jaero_batch *b, int enabled);
 int jaero_batch_get_profile(jaero_batch *b, double out[5]);
 /* Coarse-estimator path of the batch: the number of co-resident 8-CTA clusters the nfft 2^14 estimator runs on, or 0 when it
- * runs as the four-step kernels through global memory (nfft 2^13, JAERO_CFE_CLUSTER=0, or no cluster fits the device). */
+ * runs as the four-step kernels through global memory (nfft up to 2^13, or no cluster fits the device). */
 int jaero_batch_cfe_clusters(const jaero_batch *b);
 
 /* ---- test support (not part of the drop-in surface) ----
@@ -156,12 +156,13 @@ int jaero_batch_cfe_geometry(const jaero_batch *b, int32_t out[6]);
 /* Waits for the batch to be idle, copies ring[ch*bb_len + k] (complex, interleaved re/im) into the batch's baseband ring, applies
  * CoarseFreqEstimate::bigchange() to the channels with bigchange[ch] != 0 (NULL: none) as the demodulator kernels do, runs one
  * epoch linearised from ring index `oldest` and synchronises. impl: 0 the path jaero_batch_write takes, 1 the four-pass kernels,
- * 2 the cluster kernel (JAERO_E_STATE where it cannot run); max_clusters > 0 caps the clusters the cluster kernel is launched with.
+ * 2 the cluster kernel (JAERO_E_STATE where it cannot run); max_clusters > 0 caps the clusters the cluster kernel is launched with,
+ * and max_group > 0 the channels per pass group of the four-pass kernels (0: the batch's own, at most 1024).
  * y_out [n_channels][nfft] (the cluster kernel stores only bins lo-expectedpeakbin-1 .. hi+expectedpeakbin+1), raw_est [n_channels]
  * (freq_offset_est) and emitted_est [n_channels] (the gated value FreqOffsetEstimate carries) may each be NULL. Afterwards the
  * batch is in the state an estimator epoch of jaero_batch_write leaves it in, with the caller's ring as its baseband ring. */
 int jaero_batch_probe_cfe(jaero_batch *b, const double *ring, int oldest, const int32_t *bigchange, int impl, int max_clusters,
-                          double *y_out, double *raw_est, double *emitted_est);
+                          int max_group, double *y_out, double *raw_est, double *emitted_est);
 
 /* ---- K=7 r=1/2 soft Viterbi (polys 109,79), one independent decoder per channel ---- */
 int jaero_viterbi_create(int n_channels, int paddinglength, int device_ordinal, jaero_viterbi **out);

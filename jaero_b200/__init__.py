@@ -118,7 +118,7 @@ def lib():
         L.jaero_batch_get_profile.argtypes = [vp, vp]
         L.jaero_batch_cfe_clusters.argtypes = [vp]
         L.jaero_batch_cfe_geometry.argtypes = [vp, vp]
-        L.jaero_batch_probe_cfe.argtypes = [vp, vp, i, vp, i, i, vp, vp, vp]
+        L.jaero_batch_probe_cfe.argtypes = [vp, vp, i, vp, i, i, i, vp, vp, vp]
         L.jaero_viterbi_create.argtypes = [i, i, i, ctypes.POINTER(vp)]
         L.jaero_viterbi_destroy.argtypes = [vp]; L.jaero_viterbi_destroy.restype = None
         L.jaero_viterbi_decode_continuous.argtypes = [vp, vp, sz, i, vp, vp]
@@ -319,9 +319,10 @@ class DemodBatch:
         _check(lib().jaero_batch_cfe_geometry(self.h, _p(o)))
         return dict(zip(("nfft", "bb_len", "lo", "hi", "expectedpeakbin", "clusters"), (int(v) for v in o)))
 
-    def probe_cfe(self, ring, oldest, bigchange=None, impl=0, max_clusters=0):
+    def probe_cfe(self, ring, oldest, bigchange=None, impl=0, max_clusters=0, max_group=0):
         """test support: one coarse-estimator epoch on ring [n_channels, bb_len] complex (include/jaero_b200.h,
-        jaero_batch_probe_cfe); impl 0 as created, 1 four-pass kernels, 2 cluster kernel. -> (y [n, nfft], raw_est, emitted_est)"""
+        jaero_batch_probe_cfe); impl 0 as created, 1 four-pass kernels, 2 cluster kernel; max_group > 0 caps the four-pass
+        kernels' channel groups. -> (y [n, nfft], raw_est, emitted_est)"""
         g = self.cfe_geometry()
         ring = np.ascontiguousarray(ring, dtype=np.complex128)
         assert ring.shape == (self.n, g["bb_len"])
@@ -331,7 +332,7 @@ class DemodBatch:
         raw = np.zeros(self.n, dtype=np.float64)
         emitted = np.zeros(self.n, dtype=np.float64)
         _check(lib().jaero_batch_probe_cfe(self.h, _p(ring), int(oldest), None if bc is None else _p(bc), int(impl), int(max_clusters),
-                                           _p(y), _p(raw), _p(emitted)))
+                                           int(max_group), _p(y), _p(raw), _p(emitted)))
         return y, raw, emitted
 
     @property

@@ -21,8 +21,6 @@
 #include "fft_device.cuh"
 #include <cooperative_groups.h>
 #include <cstring>
-#include <cstdio>
-#include <cstdlib>
 
 namespace jb {
 
@@ -538,16 +536,7 @@ int cfe_cluster_capacity()
     cfg.attrs = &at; cfg.numAttrs = 1;
     int n = 0;
     if (cudaOccupancyMaxActiveClusters(&n, cfe_cluster_kernel, &cfg) != cudaSuccess) { cudaGetLastError(); return 0; }
-    if (getenv("JAERO_DEBUG")) fprintf(stderr, "[jaero_b200] estimator clusters co-resident: %d x %d CTAs\n", n, CC_CL);
     return n;
-}
-
-__global__ void cfe_mark_kernel(int *flag, int value) { __threadfence(); atomicExch(flag, value); }
-int cfe_mark_launch(int *flag, int value, cudaStream_t s)
-{
-    cfe_mark_kernel<<<1, 1, 0, s>>>(flag, value);
-    JB_CUDA(cudaGetLastError());
-    return 0;
 }
 
 // `oldest` = ring index of the oldest sample (the linearisation origin, oqpskdemodulator.cpp:418-424)

@@ -59,9 +59,7 @@ struct DemodParams {
     int afc, sql, cpu_reduce, report_ebno;
     int ntaps;                        // 55 (OQPSK) / 2*SPS (MSK)
     int agc_len, ebno_len, bbnfft;
-    int bb_len;                       // entries per row of the coarse-estimator ring: nfft, or 5*nfft/4 when the estimator runs
-                                      // concurrently with the next segment (the extra quarter is the one being written)
-    int *cfe_flag;                    // device counter: coarse estimates completed (asynchronous estimator only)
+    int bb_len;                       // entries per row of the coarse-estimator ring (= bbnfft)
     int marg_len, dt_len, mse_len;    // 800/401/400 (OQPSK) ; SPS / SPS/2+1 / 600 (MSK)
     int sps;                          // MSK: int(Fs/fb)
     double correctionfactor;          // MSK
@@ -106,16 +104,11 @@ struct SegmentArgs {
     int apply_cfe;                    // run FreqOffsetEstimateSlot(cfe_est_out[ch]) before anything else
     int bb_pos, coarse_counter;       // bbcycbuff_ptr, coarseCounter at entry
     int new_write;                    // first launch of a writeData call: latch lastmse
-    int cfe_wait;                     // >0: the estimate consumed by apply_cfe is produced concurrently; a channel that needs
-                                      // it waits until *cfe_flag >= cfe_wait
-    long long *trace;                 // development aid (JAERO_PIPE_TRACE): clock64 stamps of the pipeline stages of CTA 0, lane 0,
-    int trace_j0;                     // for 64 samples from loop index trace_j0 on: trace[(j-j0)*16 + stamp]; null otherwise
 };
 
 int oqpsk_segment_launch(const DemodParams &p, const SegmentArgs &a, const int16_t *d_pcm, size_t stride, cudaStream_t s);
 int oqpsk_pipe_launch(const DemodParams &p, const SegmentArgs &a, const int16_t *d_pcm, size_t stride, cudaStream_t s);
 int msk_pipe_launch(const DemodParams &p, const SegmentArgs &a, const int16_t *d_pcm, size_t stride, cudaStream_t s);
-int msk_segment_launch(const DemodParams &p, const SegmentArgs &a, const int16_t *d_pcm, size_t stride, cudaStream_t s);
 
 // K2: coarse frequency estimate for every channel of a batch (coarsefreqestimate.cpp:90-137)
 struct CfePlan {
@@ -129,7 +122,6 @@ struct CfePlan {
     int group;          // channels per pass group (sized so the work buffers stay L2-resident)
 };
 int cfe_run(const CfePlan &plan, const DemodParams &p, int oldest, cudaStream_t s, long long *launches);
-int cfe_mark_launch(int *flag, int value, cudaStream_t s);
 int cfe_cluster_run(const CfePlan &plan, const DemodParams &p, int oldest, int n_clusters, cudaStream_t s, long long *launches);
 int cfe_cluster_capacity();
 

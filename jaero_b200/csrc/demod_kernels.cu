@@ -2,5 +2,4 @@
 // Built with -fmad=false: see demod_device.cuh.
 #include "oqpsk_demod.cu"
 #include "oqpsk_pipe.cu"
-#include "msk_demod.cu"
 #include "msk_pipe.cu"

@@ -1,9 +1,9 @@
-// Stages that two or more of the continuous demodulator kernels share (oqpsk_demod.cu, oqpsk_pipe.cu, msk_demod.cu,
-// msk_pipe.cu). Each restates one piece of JAERO/oqpskdemodulator.cpp, mskdemodulator.cpp or DSP.h / DSP.cpp, in the
-// reference's operation order (see demod_device.cuh for the rounding rules).
+// Stages of the continuous demodulator kernels (oqpsk_demod.cu, oqpsk_pipe.cu, msk_pipe.cu). Each restates one piece of
+// JAERO/oqpskdemodulator.cpp, mskdemodulator.cpp or DSP.h / DSP.cpp, in the reference's operation order (see
+// demod_device.cuh for the rounding rules).
 //
-// The symbol-rate tails divide a moving sum by its length as `x / len` in the single-warp kernels and by div_exact in the
-// pipelined ones; the `Mean` policy below carries that choice, so each kernel keeps its form. The OQPSK EbNo read-out
+// The symbol-rate tails divide a moving sum by its length as `x / len` in the single-warp OQPSK kernel and by div_exact in
+// the pipelined ones; the `Mean` policy below carries that choice, so each kernel keeps its form. The OQPSK EbNo read-out
 // divides with `/` in both OQPSK kernels.
 #pragma once
 #include "demod_device.cuh"

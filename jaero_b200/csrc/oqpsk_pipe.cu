@@ -46,7 +46,6 @@ static const int PP_SM_TOTAL = PP_SM_BASE + PP_SM_HAND + PP_SM_DV + PP_SM_BBST;
 enum { BAR_X = 1, BAR_YT = 3, BAR_Z = 5, BAR_W = 7, BAR_P = 9, BAR_YK = 11, BAR_U = 13 };
 
 #define RING_WAIT(idx) do { mbar_wait(&bars[(idx)], (phases >> (idx)) & 1u); phases ^= (1u << (idx)); } while (0)
-#define TR(k) do { if (a.trace && blockIdx.x == 0 && lane == 0 && j >= a.trace_j0 && j < a.trace_j0 + 64) a.trace[(j - a.trace_j0) * 16 + (k)] = clock64(); } while (0)
 __global__ void __launch_bounds__(PP_THREADS)
 oqpsk_pipe_kernel(const __grid_constant__ DemodParams p, const SegmentArgs a, const int16_t *__restrict__ pcm, size_t stride)
 {
@@ -97,20 +96,7 @@ oqpsk_pipe_kernel(const __grid_constant__ DemodParams p, const SegmentArgs a, co
             const double mse = LD(D_MSE);
             int dcd = LI(I_DCD);
             int countdown = LI(I_COUNTDOWN), countdown2 = LI(I_COUNTDOWN2);
-            double est = 0.0;
-            if (a.cfe_wait > 0) {
-                // The estimator of this trigger runs concurrently (capi.cu). Its result only enters the arithmetic below when
-                // the channel is unlocked / has no carrier detect, and its state (y[], emptyingcountdown) is only touched by
-                // the AFC re-centre: channels in neither case proceed without it.
-                const bool recentre = (p.afc) && (mse < p.signalthreshold) && (fabs(m2.freq - mc.freq) > 3.0) && (countdown <= 0);
-                const bool need = (mse > p.signalthreshold) || (!dcd) || recentre;
-                if (__any_sync(0xffffffffu, need)) {
-                    const volatile int *flag = p.cfe_flag;
-                    while (*flag < a.cfe_wait) __nanosleep(256);
-                    __threadfence();
-                }
-                if (need) est = __ldcg(p.cfe_est_out + ch);
-            } else est = p.cfe_est_out[ch];
+            const double est = p.cfe_est_out[ch];
             if (oqpsk_freq_offset_slot(p, ch, live, est, mse, dcd, m2, mc, countdown, countdown2, LI(I_SIG_TRUE), LI(I_SIG_FALSE))) {
                 LD(D_MC_STEP) = mc.step; LD(D_MC_FREQ) = mc.freq;     // warp A reloads mixer_center after the barrier
             }
@@ -143,7 +129,6 @@ oqpsk_pipe_kernel(const __grid_constant__ DemodParams p, const SegmentArgs a, co
                 // a carrier update moves the pointer by ct_ec degrees = 55.6 * ct_ec entries: a few entries in lock, so the
                 // entry needed after an update sits in the speculated 128-byte line or one of its neighbours
                 nb_sync(BAR_P + sl);                           // P_j: carrier error of this sample (warp K1)
-                TR(8);
                 const double upd = HAND(sl, 14), ct_ec = HAND(sl, 15);
                 if (upd != 0.0) {                                                 // :518-525, fb > 8400 (the host only uses this kernel there)
                     osc_increase_phase_deg(m2, 1.0 * ct_ec);
@@ -154,11 +139,9 @@ oqpsk_pipe_kernel(const __grid_constant__ DemodParams p, const SegmentArgs a, co
                     const int t = osc_index(m2.ptr);
                     if (t == m2_spec) { c2_re = n2_re; c2_im = n2_im; } else { c2_re = __ldcg(cos_t + t); c2_im = __ldcg(sin_t + t); }
                 }
-                TR(13);
                 if (j + 1 < nB) {   // the next sample's mixed value enters the FIR ring (:453-456)
                     fir_push2(s_re, s_im, OQ_NT1, lane, fir_pos, c2_re * dnext, c2_im * dnext);
                     handoff(BAR_X + ((j + 1) & 1));            // X_{j+1}
-                    TR(9);
                 }
             }
         }
@@ -183,7 +166,6 @@ oqpsk_pipe_kernel(const __grid_constant__ DemodParams p, const SegmentArgs a, co
                 double2 sig2 = make_double2(HAND(sl, 2), HAND(sl, 3));
                 nb_sync(BAR_U + sl);                           // strobe decision of this sample (warp T)
                 const double strobe = HAND(sl, 10), frac = HAND(sl, 11);
-                TR(6);
                 if (!sig2l_init) { sig2_last = sig2; sig2l_init = 1; }            // :487 static initialiser
                 double sy_flag = 0.0, sy_x = 0.0, sy_y = 0.0, sy_ec = 0.0, k2_upd = 0.0, k2_ec = 0.0;
                 if (strobe != 0.0) {                                              // :488
@@ -210,7 +192,6 @@ oqpsk_pipe_kernel(const __grid_constant__ DemodParams p, const SegmentArgs a, co
                 // slot sl's K1->K2 fields were read by K2(j-2), which precedes X_{j-1} -> ... -> U_j: free
                 HAND(sl, 14) = k2_upd; HAND(sl, 15) = k2_ec;
                 handoff(BAR_P + sl);                           // P_j
-                TR(7);
                 // symbol hand-off to warp S; slot reuse is gated by S's arrival on the slot's mbarrier
                 if (j >= 2) { mbar_wait(&bars[5 + sl], (vph >> sl) & 1u); vph ^= (1u << sl); }
                 HAND(sl, 6) = sy_x; HAND(sl, 7) = sy_y; HAND(sl, 8) = sy_ec; HAND(sl, 9) = sy_flag;
@@ -256,10 +237,8 @@ oqpsk_pipe_kernel(const __grid_constant__ DemodParams p, const SegmentArgs a, co
             const double ns_re = cos_t[st_spec], ns_im = sin_t[st_spec];
             nb_sync(BAR_YT + sl);                              // st_eta, d8out of this sample (warp E)
             const double st_eta = HAND(sl, 4), d8out = HAND(sl, 5);
-            TR(4);
             const double2 st_out = cmul(make_double2(cs_re, cs_im), make_double2(st_eta, -d8out));   // :478-479
             const double st_angle_error = atan2_fast(st_out.y, st_out.x);     // :480 std::arg
-            TR(11);
             osc_set_freq(st, (-st_angle_error * 0.00000001) + st.freq, Fs);   // :481 IncreseFreqHz
             osc_advance_fraction_of_wave(st, div_exact(-st_angle_error * 0.01, 360.0, 1.0 / 360.0)); // :482
             if (st.freq < (sr_freq - 0.1)) osc_set_freq(st, (sr_freq - 0.1), Fs);
@@ -269,7 +248,6 @@ oqpsk_pipe_kernel(const __grid_constant__ DemodParams p, const SegmentArgs a, co
             // slot sl's T->K1 fields were read by K1(j-2), which precedes X_{j-1} -> Z_j -> (E) -> this point: free
             HAND(sl, 10) = strobe ? 1.0 : 0.0; HAND(sl, 11) = frac;
             handoff(BAR_U + sl);
-            TR(5);
             osc_next_frame(st);                                               // :602 (st_osc_ref, :603, advances in warp A)
             { const int t = osc_index(st.ptr); if (t == st_spec) { cs_re = ns_re; cs_im = ns_im; } else { cs_re = cos_t[t]; cs_im = sin_t[t]; } }
         }
@@ -347,7 +325,6 @@ oqpsk_pipe_kernel(const __grid_constant__ DemodParams p, const SegmentArgs a, co
                 p8++; if (p8 > k8) p8 = 0;
                 nb_sync(BAR_Z + sl);                           // Z_j: FIR output of this sample
                 const double sre = HAND(sl, 0), sim = HAND(sl, 1);
-                TR(2);
                 const double dabval = sqrt(sre * sre + sim * sim);                // :461
                 if (ebno_on) {                                                    // OQPSKEbNoMeasure::Update (DSP.cpp:729-744)
                     const double sq = dabval * dabval;
@@ -363,7 +340,6 @@ oqpsk_pipe_kernel(const __grid_constant__ DemodParams p, const SegmentArgs a, co
                 }
                 double2 sig2 = make_double2(sre * agc_val, sim * agc_val);        // :466
                 const double abval = hypot_fast(sig2.x, sig2.y);                  // :469 std::abs
-                TR(10);
                 if (abval > 2.84) { const double g = (2.84 / abval); sig2 = make_double2(g * sig2.x, g * sig2.y); }   // :470
                 // ---- symbol timing, feed-forward part (:473-477)
                 const double ab2 = abval * abval;
@@ -395,7 +371,6 @@ oqpsk_pipe_kernel(const __grid_constant__ DemodParams p, const SegmentArgs a, co
                 HAND(sl, 2) = sig2.x; HAND(sl, 3) = sig2.y; HAND(sl, 4) = st_eta; HAND(sl, 5) = d8out;
                 handoff(BAR_YT + sl);                          // timing inputs -> warp T
                 nb_arrive(BAR_YK + sl);                        // sig2 -> warp K
-                TR(3);
                 // ---- ring tile bookkeeping (warp-uniform)
                 S++;
                 if ((S & (OQ_T - 1)) == 0) {
@@ -438,12 +413,10 @@ oqpsk_pipe_kernel(const __grid_constant__ DemodParams p, const SegmentArgs a, co
         for (int j = 0; j < nB; j++) {
             const int sl = j & 1;
             if (j > 0) nb_sync(BAR_X + ((j - 1) & 1));        // X_{j-1}
-            TR(0);
             nfre += p.taps[54] * s_re[tail * 32 + lane]; nfim += p.taps[54] * s_im[tail * 32 + lane];
             // slot sl's F->E fields were read by E(j-2), before X_{j-1}: free
             HAND(sl, 0) = nfre; HAND(sl, 1) = nfim;
             handoff(BAR_Z + sl);                               // Z_j
-            TR(1);
             tail++; if (tail >= OQ_NT1) tail = 0;
             if (j + 1 < nB) fir54(p, s_re + (tail + 2) * 32 + lane, s_im + (tail + 2) * 32 + lane, nfre, nfim);
         }
@@ -514,4 +487,3 @@ int oqpsk_pipe_launch(const DemodParams &p, const SegmentArgs &a, const int16_t 
 } // namespace jb
 
 #undef RING_WAIT
-#undef TR

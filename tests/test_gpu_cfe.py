@@ -1,13 +1,11 @@
 """GPU tests of the coarse frequency estimator kernels (pytest -m gpu) against the long-double restatement of
 CoarseFreqEstimate::ProcessBasebandData in tests/cfe_reference.py, one epoch at a time through jaero_batch_probe_cfe: the
 four-pass kernels at every FFT size and the cluster kernel at 2^14, channel groups, cluster reuse across channels, the general
-fold-search path, the asynchronous ring, odd channel counts; then whole recordings under every estimator switch against the
-CPU oracle's per-epoch estimates.
+fold-search path, odd channel counts; then whole recordings against the CPU oracle's per-epoch estimates.
 
 Each epoch checks the spectrum max(|X|,1) recovered from the smoothed y against the long-double value, the fold search on the
 kernel's own y against the restated loop (exactly), the estimate against the reference (near-ties counted and skipped), and the
 emit gate."""
-import contextlib
 import functools
 import os
 
@@ -23,34 +21,18 @@ pytestmark = [pytest.mark.gpu, pytest.mark.skipif(not has_cuda(), reason="needs 
 FOUR_PASS, CLUSTER = 1, 2
 
 
-@contextlib.contextmanager
-def switches(**kw):
-    """environment switches are read when a batch is created: set them around the create, restore them afterwards"""
-    old = {k: os.environ.get(k) for k in kw}
-    os.environ.update({k: str(v) for k, v in kw.items()})
-    try:
-        yield
-    finally:
-        for k, v in old.items():
-            if v is None:
-                os.environ.pop(k, None)
-            else:
-                os.environ[k] = v
-
-
 def default_flags(C):
     """bigchange() before epoch 0 on every third channel (the all-zero channel among them) and mid-sequence on others"""
     c = np.arange(C)
     return {0: c % 3 == 0, 3: c % 3 == 1}
 
 
-def run_epochs(kind, fb, lockingbw, power, C, runs, epochs=8, flags=None, env=None, seed=0, oldest_extra=()):
+def run_epochs(kind, fb, lockingbw, power, C, runs, epochs=8, flags=None, max_group=0, seed=0):
     """runs: list of (impl, max_clusters); one batch per run, all fed the same rings. Returns the checkers."""
     import jaero_b200
     g = R.geometry(power, lockingbw, fb)
     N = g["nfft"]
-    with switches(**(env or {})):
-        batches = [jaero_b200.DemodBatch(kind, C, fb=fb, lockingbw=lockingbw, fft_power=power) for _ in runs]
+    batches = [jaero_b200.DemodBatch(kind, C, fb=fb, lockingbw=lockingbw, fft_power=power) for _ in runs]
     geo = batches[0].cfe_geometry()
     assert (geo["nfft"], geo["lo"], geo["hi"], geo["expectedpeakbin"]) == (N, g["lo"], g["hi"], g["expectedpeakbin"])
     bb_len = geo["bb_len"]
@@ -62,7 +44,7 @@ def run_epochs(kind, fb, lockingbw, power, C, runs, epochs=8, flags=None, env=No
     ties = [c for c in range(C) if kinds[c] in R.TIE_KINDS]
     orc = {c: restated.OracleCfe(power, lockingbw, fb) for c in ties}
     flags = default_flags(C) if flags is None else flags
-    oldests = [0, 1, None, bb_len - 1] + list(oldest_extra)
+    oldests = [0, 1, None, bb_len - 1]
     try:
         for e in range(epochs):
             oldest = oldests[e % len(oldests)]
@@ -79,7 +61,7 @@ def run_epochs(kind, fb, lockingbw, power, C, runs, epochs=8, flags=None, env=No
             out = ref.process(data)
             for (impl, mc), b, chk in zip(runs, batches, checkers):
                 what = "%s fb %g 2^%d C=%d impl %d clusters %d epoch %d oldest %d" % (kind, fb, power, C, impl, mc, e, oldest)
-                y, raw, emitted = b.probe_cfe(ring, oldest, bc.astype(np.int32), impl=impl, max_clusters=mc)
+                y, raw, emitted = b.probe_cfe(ring, oldest, bc.astype(np.int32), impl=impl, max_clusters=mc, max_group=max_group)
                 chk.epoch(out, y, raw, bc, kinds, tie_raw=tie_raw, what=what)
                 gate = np.where(out["gate_open"], raw, 0.0)
                 assert np.array_equal(emitted, gate), "%s: emitted %r, gate says %r" % (what, emitted, gate)
@@ -91,8 +73,8 @@ def run_epochs(kind, fb, lockingbw, power, C, runs, epochs=8, flags=None, env=No
         for o in orc.values():
             o.close()
     for (impl, mc), chk in zip(runs, checkers):
-        print("CFE-STATS %s fb=%g 2^%d C=%d impl=%d clusters=%d env=%s: compared %d, near-tie skips %d, worst spectrum error %.3g of the bound"
-              % (kind, fb, power, C, impl, mc, env or {}, chk.compared, chk.skips, chk.worst))
+        print("CFE-STATS %s fb=%g 2^%d C=%d impl=%d clusters=%d group=%d: compared %d, near-tie skips %d, worst spectrum error %.3g of the bound"
+              % (kind, fb, power, C, impl, mc, max_group, chk.compared, chk.skips, chk.worst))
         assert chk.skips <= max(1, 0.02 * chk.compared), (chk.skips, chk.compared, chk.skipped_kinds)
         assert chk.compared >= epochs * C * 0.9
     return checkers
@@ -111,10 +93,10 @@ def test_estimator_matches_long_double_reference(kind, fb, lockingbw, power):
 
 
 def test_channel_groups_offset_every_per_channel_array():
-    """JAERO_CFE_GROUP=16 at 70 channels: four full groups and a ragged one; bigchange() on both sides of every group boundary"""
+    """groups of 16 at 70 channels: four full groups and a ragged one; bigchange() on both sides of every group boundary"""
     C = 70
     flags = {0: np.isin(np.arange(C), [0, 15, 32, 47, 64, 69]), 3: np.isin(np.arange(C), [16, 31, 48, 63, 1])}
-    run_epochs("oqpsk", 10500.0, 10500.0, 13, C, [(FOUR_PASS, 0)], flags=flags, env=dict(JAERO_CFE_GROUP=16))
+    run_epochs("oqpsk", 10500.0, 10500.0, 13, C, [(FOUR_PASS, 0)], flags=flags, max_group=16)
 
 
 def test_cluster_kernel_reuses_its_clusters_across_channels():
@@ -134,19 +116,6 @@ def test_fold_search_general_path(power):
     g = R.geometry(power, 20000.0, 10500.0)
     assert g["lo"] - g["expectedpeakbin"] - 1 < 0 or g["hi"] + g["expectedpeakbin"] + 1 >= g["nfft"]
     run_epochs("oqpsk", 10500.0, 20000.0, power, 7, [(FOUR_PASS, 0)] + ([(CLUSTER, 0)] if power == 14 else []))
-
-
-def test_async_estimator_ring():
-    """JAERO_ASYNC_CFE=1: the ring is 1.25 nfft long; linearisation origins near its wrap"""
-    import jaero_b200
-    with switches(JAERO_ASYNC_CFE=1):
-        b = jaero_b200.DemodBatch("oqpsk", 7, fb=10500.0)
-    geo = b.cfe_geometry()
-    b.close()
-    assert geo["bb_len"] == geo["nfft"] + geo["nfft"] // 4, "the asynchronous estimator is not enabled"
-    n = geo["bb_len"]
-    run_epochs("oqpsk", 10500.0, 10500.0, 14, 7, [(0, 0), (FOUR_PASS, 0)], env=dict(JAERO_ASYNC_CFE=1),
-               oldest_extra=(n - 2, n - geo["nfft"] // 4, n - geo["nfft"] // 4 - 1, n - 17))
 
 
 @pytest.mark.parametrize("C", [1, 5])
@@ -181,49 +150,33 @@ def _oracle_estimates(name):
     return case["kind"], kw, pcm, raw, emitted
 
 
-def _gpu_estimates(name, env):
+def _gpu_estimates(name):
     import jaero_b200
     kind, kw, pcm, _, _ = _oracle_estimates(name)
     quarter = (1 << kw["fft_power"]) // 4
-    with switches(**env):
-        b = jaero_b200.DemodBatch(kind, 3, **kw)
+    b = jaero_b200.DemodBatch(kind, 3, **kw)
     geo = b.cfe_geometry()
-    ests, soft = [], [[] for _ in range(3)]
+    ests = []
     try:
         for a in range(0, pcm.shape[1], quarter):
             b.write(pcm[:, a:a + quarter])                        # exactly one estimator epoch per call
             ests.append([s["cfe_est"] for s in b.status()])
-            for c, s in enumerate(b.read_softbits()):
-                soft[c].append(s)
     finally:
         b.close()
-    return geo, np.asarray(ests).T, [np.concatenate(s) for s in soft]
+    return geo, np.asarray(ests).T
 
 
-@pytest.mark.parametrize("name,env", [
-    ("oqpsk_10500", {}), ("oqpsk_10500", dict(JAERO_CFE_CLUSTER=0)), ("oqpsk_10500", dict(JAERO_CFE_CLUSTER=0, JAERO_CFE_GROUP=2)),
-    ("oqpsk_10500", dict(JAERO_ASYNC_CFE=1)),
-    ("oqpsk_8400", {}), ("oqpsk_8400", dict(JAERO_CFE_CLUSTER=0)), ("oqpsk_8400", dict(JAERO_CFE_CLUSTER=0, JAERO_CFE_GROUP=2)),
-    ("msk_1200", {}), ("msk_1200", dict(JAERO_CFE_CLUSTER=0)), ("msk_1200", dict(JAERO_CFE_CLUSTER=0, JAERO_CFE_GROUP=2)),
-])
-def test_recording_estimates_per_epoch(name, env):
-    """3 channels of a recording, one trigger interval per write: the estimate of every epoch equals the oracle's, under every
-    estimator switch; the asynchronous estimator leaves the soft bits unchanged"""
+@pytest.mark.parametrize("name", ["oqpsk_10500", "oqpsk_8400", "msk_1200"])
+def test_recording_estimates_per_epoch(name):
+    """3 channels of a recording, one trigger interval per write: the estimate of every epoch equals the oracle's (the cluster
+    kernel at nfft 2^14, the four-pass kernels below it)"""
     _, _, pcm, raw, emitted = _oracle_estimates(name)
-    geo, got, soft = _gpu_estimates(name, env)
-    if env.get("JAERO_CFE_CLUSTER") == 0:
-        assert geo["clusters"] == 0
-    elif geo["nfft"] == 16384:
+    geo, got = _gpu_estimates(name)
+    if geo["nfft"] == 16384:
         assert geo["clusters"] > 0
-    if "JAERO_ASYNC_CFE" in env:
-        assert geo["bb_len"] == geo["nfft"] + geo["nfft"] // 4
     for c in range(3):
         assert len(raw[c]) == got.shape[1] and len(raw[c]) > 50
         bad = np.nonzero(got[c] != raw[c])[0]
-        assert len(bad) == 0, "%s %s channel %d: epochs %s differ, gpu %s, oracle %s" % (name, env, c, bad[:8], got[c][bad[:4]], raw[c][bad[:4]])
+        assert len(bad) == 0, "%s channel %d: epochs %s differ, gpu %s, oracle %s" % (name, c, bad[:8], got[c][bad[:4]], raw[c][bad[:4]])
         nz = emitted[c] != 0                                      # what the oracle emitted past the gate is that epoch's estimate
         assert np.array_equal(emitted[c][nz], raw[c][nz])
-    if "JAERO_ASYNC_CFE" in env:
-        _, _, soft_default = _gpu_estimates(name, {})
-        for c in range(3):
-            assert np.array_equal(soft[c], soft_default[c]), c

@@ -1,7 +1,7 @@
 """GPU test (pytest -m gpu): the cluster-resident coarse estimator returns, bit for bit, the smoothed spectrum y, raw estimate and
 emitted estimate recorded in tests/golden/cfe_cluster_digests.json (tools/make_cfe_digests.py) for every epoch of seeded rings:
-both spectrum shapes, few clusters for many channels, more channels than twice the device's cluster capacity, bigchange() before
-the first and in a later epoch, and the asynchronous estimator's longer ring."""
+both spectrum shapes, few clusters for many channels, more channels than twice the device's cluster capacity, and bigchange()
+before the first and in a later epoch."""
 import importlib.util
 import json
 import os

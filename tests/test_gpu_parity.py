@@ -172,6 +172,22 @@ def test_oqpsk_parity_synthetic_ebn0_sweep(ebn0):
     assert sum(len(s) for s in soft_g) > 10000
 
 
+def test_oqpsk_parity_below_8400_bps():
+    """OQPSK rates below 8400 bps other than 8400 itself run the single-warp kernel without the pre-filter: 8000 bps at
+    48 kHz, on a synthetic 8000 bps signal and on the 10.5 kbps recording."""
+    from jaero_b200 import synth
+    rng = np.random.default_rng(8000)
+    env = synth.oqpsk_envelope(rng.integers(0, 2, size=8000 * 6, dtype=np.uint8), 8000.0)
+    pcm2 = np.stack([synth.to_passband_int16(env, 6000.0, ebn0_db=12.0, fb=8000.0, rng=rng),
+                     load_excerpt("oqpsk_10500")[:len(env)]])
+    kw = dict(fb=8000, freq_center=6000.0, lockingbw=8000, fft_power=14, signalthreshold=0.65, afc=True)
+    soft_g, st_g = _run_gpu("oqpsk", pcm2, kw, 6000)
+    for c in range(2):
+        soft_o, st_o = _run_oracle("oqpsk", pcm2[c], kw, 6000)
+        _assert_parity(soft_g[c], st_g[c], soft_o, st_o)
+    assert len(soft_g[0]) > 10000
+
+
 def test_msk1200_parity_synthetic_cfg2():
     """BASELINE cfg 2 signal model (continuous 1200 bps MSK P-channel, Eb/N0 = 8 dB, carriers 2000 +- 200 Hz, random phase and
     timing): soft bits / loop state against the oracle, then the device P-channel layer against the oracle's, DCD fed back on

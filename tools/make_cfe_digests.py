@@ -19,16 +19,15 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 OUT = os.path.join(ROOT, "tests", "golden", "cfe_cluster_digests.json")
 
 EPOCHS = 6
-# name -> (fb, channels, max_clusters, JAERO_ASYNC_CFE). "wide" has more than twice as many channels as an H100 can hold
-# clusters of the kernel, so every cluster runs several channels in turn.
+# name -> (fb, channels, max_clusters). "wide" has more than twice as many channels as an H100 can hold clusters of the
+# kernel, so every cluster runs several channels in turn.
 CASES = {
-    "10500_c7": (10500.0, 7, 0, 0),
-    "8400_c7": (8400.0, 7, 0, 0),
-    "10500_c20_mc1": (10500.0, 20, 1, 0),
-    "10500_c20_mc2": (10500.0, 20, 2, 0),
-    "10500_c20_mc7": (10500.0, 20, 7, 0),
-    "8400_wide": (8400.0, 160, 0, 0),
-    "10500_async_c7": (10500.0, 7, 0, 1),
+    "10500_c7": (10500.0, 7, 0),
+    "8400_c7": (8400.0, 7, 0),
+    "10500_c20_mc1": (10500.0, 20, 1),
+    "10500_c20_mc2": (10500.0, 20, 2),
+    "10500_c20_mc7": (10500.0, 20, 7),
+    "8400_wide": (8400.0, 160, 0),
 }
 
 
@@ -40,17 +39,9 @@ def run_case(name):
     """-> dict(clusters=co-resident clusters of the batch, epochs=[dict(y, raw, emitted) digests per epoch])"""
     import cfe_reference as R
     import jaero_b200
-    fb, C, max_clusters, asynchronous = CASES[name]
+    fb, C, max_clusters = CASES[name]
     lockingbw = 10500.0
-    old = os.environ.get("JAERO_ASYNC_CFE")
-    os.environ["JAERO_ASYNC_CFE"] = str(asynchronous)
-    try:
-        b = jaero_b200.DemodBatch("oqpsk", C, fb=fb, lockingbw=lockingbw, fft_power=14)
-    finally:
-        if old is None:
-            os.environ.pop("JAERO_ASYNC_CFE")
-        else:
-            os.environ["JAERO_ASYNC_CFE"] = old
+    b = jaero_b200.DemodBatch("oqpsk", C, fb=fb, lockingbw=lockingbw, fft_power=14)
     try:
         geo = b.cfe_geometry()
         n = geo["bb_len"]
@@ -59,7 +50,7 @@ def run_case(name):
         offsets = rng.uniform(-0.4, 0.4, C) * lockingbw / 2
         c = np.arange(C)
         flags = {0: c % 3 == 0, 3: c % 3 == 1}                  # bigchange() before epoch 0 and mid-sequence
-        oldests = [0, 1, None, n - 1, n - 2, n - 17]            # the last ones cross the wrap of the 1.25 nfft asynchronous ring
+        oldests = [0, 1, None, n - 1, n - 2, n - 17]            # the last ones cross the wrap of the ring
         epochs = []
         for e in range(EPOCHS):
             oldest = oldests[e % len(oldests)]
