@@ -22,6 +22,7 @@ UNITS = [
     ("ddc.cu", []),
     ("scan.cu", []),
     ("prefilter.cu", ["-fmad=false"]),
+    ("fastfir.cu", ["-fmad=false"]),
     ("burst.cu", ["-fmad=false"]),
     ("demod_kernels.cu", ["-fmad=false"]),
 ]

@@ -3,7 +3,8 @@
 // Replaces BurstMskDemodulator::writeData (JAERO/burstmskdemodulator.cpp:371-754) and the primitives only it uses
 // (QJHilbertFilter DSP.cpp:754-794 over JFastFir, TMovingAverage DSP.h:145-199, PeakDetector DSP.h:491-576,
 // FFTrWrapper fftrwrapper.cpp:19-27). One internal chunk (<= BURST_CHUNK samples) runs as
-//   hilbert_*        streaming FFT-8192 convolution with the 2048-tap Hilbert kernel -> analytic signal
+//   hilbert_exchange thread/channel: the sample exchange of the streaming FFT convolution (fastfir.cuh, nfft 8192) with the
+//                    2048-tap Hilbert kernel, PCM in -> analytic signal out; its block kernel is the shared one of fastfir.cu
 //   burst_front      thread/channel, always active: AGC(1 s), alignment delays d1/d2, burst-timing statistic
 //                    (delay-conjugate-multiply -> MA -> MA -> minus delayed copy -> square), PeakDetector, trident-buffer
 //                    fills; every completed fill is recorded as an event (sample index + buffer slot)
@@ -19,35 +20,12 @@
 
 namespace jb {
 
-
 #define BD(idx) p.BD[(size_t)(idx) * p.cpad + ch]
 #define BI(idx) p.BI[(size_t)(idx) * p.cpad + ch]
 
 // ------------------------------------------------------------------------------------------------ FFT helpers
-__device__ __forceinline__ double2 b_add(double2 a, double2 b) { return make_double2(a.x + b.x, a.y + b.y); }
-__device__ __forceinline__ double2 b_sub(double2 a, double2 b) { return make_double2(a.x - b.x, a.y - b.y); }
-__device__ __forceinline__ double2 b_mul(double2 a, double2 b) { return make_double2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }
-template <bool INV> __device__ __forceinline__ double2 b_rot(double2 a) { return INV ? make_double2(-a.y, a.x) : make_double2(a.y, -a.x); }
-template <bool INV> __device__ __forceinline__ void b_dft4(double2 &a0, double2 &a1, double2 &a2, double2 &a3)
-{
-    const double2 t0 = b_add(a0, a2), t1 = b_sub(a0, a2), t2 = b_add(a1, a3), t3 = b_rot<INV>(b_sub(a1, a3));
-    a0 = b_add(t0, t2); a1 = b_add(t1, t3); a2 = b_sub(t0, t2); a3 = b_sub(t1, t3);
-}
-template <bool INV> __device__ __forceinline__ void b_dft8(double2 *v)
-{
-    double2 e0 = v[0], e1 = v[2], e2 = v[4], e3 = v[6], o0 = v[1], o1 = v[3], o2 = v[5], o3 = v[7];
-    b_dft4<INV>(e0, e1, e2, e3);
-    b_dft4<INV>(o0, o1, o2, o3);
-    const double h = 0.70710678118654752440;
-    const double2 w1 = INV ? make_double2(h, h) : make_double2(h, -h);
-    const double2 w3 = INV ? make_double2(-h, h) : make_double2(-h, -h);
-    o1 = b_mul(o1, w1); o2 = b_rot<INV>(o2); o3 = b_mul(o3, w3);
-    v[0] = b_add(e0, o0); v[4] = b_sub(e0, o0);
-    v[1] = b_add(e1, o1); v[5] = b_sub(e1, o1);
-    v[2] = b_add(e2, o2); v[6] = b_sub(e2, o2);
-    v[3] = b_add(e3, o3); v[7] = b_sub(e3, o3);
-}
-// Stockham radix-8 pass src -> dst over an n-point sequence (n a multiple of 8), any number of threads
+// Stockham radix-8 pass src -> dst over an n-point sequence (n a multiple of 8), any number of threads: the trident FFTs'
+// ping-pong through HBM (the butterfly is dft8 of fft_device.cuh)
 template <bool INV> __device__ __forceinline__ void pass8(const double2 *src, double2 *dst, int n, int Ns, const double2 *__restrict__ tw, int tw_stride)
 {
     const int nb = n >> 3;
@@ -61,32 +39,18 @@ template <bool INV> __device__ __forceinline__ void pass8(const double2 *src, do
         for (int t = 1; t < 8; t++) {
             double2 w = tw[t * k * wmul];
             if (INV) w.y = -w.y;
-            v[t] = b_mul(v[t], w);
+            v[t] = c_mul(v[t], w);
         }
-        b_dft8<INV>(v);
+        dft8<INV>(v);
         const int ob = (j / Ns) * Ns * 8 + k;
 #pragma unroll
         for (int t = 0; t < 8; t++) dst[ob + t * Ns] = v[t];
     }
 }
-template <bool INV> __device__ __forceinline__ void pass2(const double2 *src, double2 *dst, int n, int Ns, const double2 *__restrict__ tw, int tw_stride)
-{
-    const int nb = n >> 1;
-    const int wmul = tw_stride * (n / (Ns * 2));
-    for (int j = threadIdx.x; j < nb; j += blockDim.x) {
-        const int k = j % Ns;
-        double2 a = src[j], b = src[j + nb];
-        double2 w = tw[k * wmul];
-        if (INV) w.y = -w.y;
-        b = b_mul(b, w);
-        const int ob = (j / Ns) * Ns * 2 + k;
-        dst[ob] = b_add(a, b); dst[ob + Ns] = b_sub(a, b);
-    }
-}
 
 // ------------------------------------------------------------------------------------------------ Hilbert (FFT-8192 FIR)
 // JFastFir::update sample exchange: out[i] = previous block's result, staging block <- real PCM sample
-__global__ void hilbert_exchange_kernel(HilbertStream h, BurstParams p, const int16_t *__restrict__ pcm, size_t stride, int pcm0, int i0, int i1, int fill0)
+__global__ void hilbert_exchange_kernel(FastFir h, BurstParams p, const int16_t *__restrict__ pcm, size_t stride, int pcm0, int i0, int i1, int fill0)
 {
     const int ch = blockIdx.x * blockDim.x + threadIdx.x;
     if (ch >= p.n_channels) return;
@@ -101,81 +65,6 @@ __global__ void hilbert_exchange_kernel(HilbertStream h, BurstParams p, const in
         fill++;
     }
 }
-// overlap-save block in shared memory: [K-1 history | L new] -> FFT8192 -> xH -> IFFT -> last L outputs
-__global__ void __launch_bounds__(1024)
-hilbert_block_kernel(HilbertStream h, int first_block)
-{
-    extern __shared__ double2 hs[];                     // 2 x 8192 double2 would not fit: ping-pong between smem and HBM scratch
-    const int ch = blockIdx.x;
-    const int K1 = h.K - 1, L = h.L, N = h.nfft;
-    double2 *hist = h.hist + (size_t)ch * K1, *inb = h.inblk + (size_t)ch * L, *outb = h.outblk + (size_t)ch * L;
-    for (int j = threadIdx.x; j < N; j += blockDim.x) hs[j] = (j < K1) ? hist[j] : inb[j - K1];
-    __syncthreads();
-    for (int j = threadIdx.x; j < K1; j += blockDim.x) hist[j] = hs[L + j];   // last K-1 samples of the concatenation
-    __syncthreads();
-    // 8192 = 8*8*8*8*2: in-place passes need the read-all / write-all split; one butterfly per thread for the radix-8 passes
-    for (int Ns = 1; Ns <= 512; Ns *= 8) {
-        double2 v[8];
-        const int j = threadIdx.x, nb = N >> 3;
-#pragma unroll
-        for (int t = 0; t < 8; t++) v[t] = hs[j + t * nb];
-        __syncthreads();
-        const int k = j % Ns, wmul = N / (Ns * 8);
-#pragma unroll
-        for (int t = 1; t < 8; t++) v[t] = b_mul(v[t], h.tw[t * k * wmul]);
-        b_dft8<false>(v);
-        const int ob = (j / Ns) * Ns * 8 + k;
-#pragma unroll
-        for (int t = 0; t < 8; t++) hs[ob + t * Ns] = v[t];
-        __syncthreads();
-    }
-    {   // radix-2, Ns = 4096: 4 butterflies per thread
-        double2 a[4], b[4];
-        for (int q = 0; q < 4; q++) { const int j = threadIdx.x + q * 1024; a[q] = hs[j]; b[q] = hs[j + 4096]; }
-        __syncthreads();
-        for (int q = 0; q < 4; q++) {
-            const int j = threadIdx.x + q * 1024;                 // k = j (Ns = 4096), twiddle step 1
-            const double2 bw = b_mul(b[q], h.tw[j]);
-            hs[j] = b_add(a[q], bw); hs[j + 4096] = b_sub(a[q], bw);
-        }
-        __syncthreads();
-    }
-    for (int j = threadIdx.x; j < N; j += blockDim.x) hs[j] = b_mul(hs[j], h.H[j]);
-    __syncthreads();
-    for (int Ns = 1; Ns <= 512; Ns *= 8) {
-        double2 v[8];
-        const int j = threadIdx.x, nb = N >> 3;
-#pragma unroll
-        for (int t = 0; t < 8; t++) v[t] = hs[j + t * nb];
-        __syncthreads();
-        const int k = j % Ns, wmul = N / (Ns * 8);
-#pragma unroll
-        for (int t = 1; t < 8; t++) { double2 w = h.tw[t * k * wmul]; w.y = -w.y; v[t] = b_mul(v[t], w); }
-        b_dft8<true>(v);
-        const int ob = (j / Ns) * Ns * 8 + k;
-#pragma unroll
-        for (int t = 0; t < 8; t++) hs[ob + t * Ns] = v[t];
-        __syncthreads();
-    }
-    {
-        double2 a[4], b[4];
-        for (int q = 0; q < 4; q++) { const int j = threadIdx.x + q * 1024; a[q] = hs[j]; b[q] = hs[j + 4096]; }
-        __syncthreads();
-        for (int q = 0; q < 4; q++) {
-            const int j = threadIdx.x + q * 1024;
-            double2 w = h.tw[j]; w.y = -w.y;
-            const double2 bw = b_mul(b[q], w);
-            hs[j] = b_add(a[q], bw); hs[j + 4096] = b_sub(a[q], bw);
-        }
-        __syncthreads();
-    }
-    const double sc = 1.0 / (double)N;
-    for (int j = threadIdx.x; j < L; j += blockDim.x) {
-        const double2 y = hs[K1 + j];
-        outb[j] = first_block ? make_double2(0.0, 0.0) : make_double2(y.x * sc, y.y * sc);
-    }
-}
-
 // ------------------------------------------------------------------------------------------------ front end
 // Everything in front of the trident test is feed-forward (AGC -> alignment delays -> burst-timing statistic -> peak
 // detector), but every stage is a running sum or a delay line over a long ring in HBM: ten "value written len samples ago"
@@ -288,7 +177,7 @@ burst_front_kernel(BurstParams p, long long sample0, int n)
                 dly = make_double2(w * newer.x + (1.0 - w) * older.x, w * newer.y + (1.0 - w) * older.y);
                 btd1_pos++; if (btd1_pos >= p.btd1_len) btd1_pos = 0;
             }
-            const double2 prod = b_mul(cval, make_double2(dly.x, -dly.y));     // cval*std::conj(...)
+            const double2 prod = c_mul(cval, make_double2(dly.x, -dly.y));     // cval*std::conj(...)
             double2 mav;                                                       // bt_ma1.UpdateSigned (TMovingAverage<cpx>)
             {
                 const double2 old = s2[3 * BF_T];
@@ -578,10 +467,10 @@ burst_back_kernel(const __grid_constant__ BurstParams p, int n)
             { int tp = fir_pos; for (int k = 0; k < p.ntaps; k++) { sre += p.taps[k] * s_re[tp * 32 + lane]; sim += p.taps[k] * s_im[tp * 32 + lane]; tp++; if (tp >= nt1) tp = 0; } }
             double2 sig2 = make_double2(sre, sim);
             if (cntr > (p.start_processing * sps) && cntr < p.end_rotation) {       // :606-626 preamble symbol tone
-                double2 spt = cmul(cmul(sig2, strot), make_double2(0.0, 1.0));
+                double2 spt = c_mul(c_mul(sig2, strot), make_double2(0.0, 1.0));
                 const double er = tanh(spt.y) * (spt.x);
                 const double ang = (1.0 * er) * 0.5;                     // imag*er*0.5
-                strot = cmul(strot, make_double2(cos(ang), sin(ang)));
+                strot = c_mul(strot, make_double2(cos(ang), sin(ang)));
                 savrot = make_double2(savrot.x * 0.999 + 0.001 * strot.x, savrot.y * 0.999 + 0.001 * strot.y);
                 double a1out;                                             // a1.update(symboltone_pt.real()): Delay<double>(SPS/2)
                 {
@@ -597,15 +486,15 @@ burst_back_kernel(const __grid_constant__ BurstParams p, int n)
                 const double goal = p.end_rotation - (sps * p.start_processing);
                 progress = progress / goal;
                 const int th = osc_index(sh.ptr);
-                const double2 q = cmul(make_double2(p.cos_t[th], p.sin_t[th]), make_double2(spt.x, -spt.y));
+                const double2 q = c_mul(make_double2(p.cos_t[th], p.sin_t[th]), make_double2(spt.x, -spt.y));
                 double st_err = atan2(q.y, q.x);
                 st_err *= 0.5 * (1.0 - progress * progress);
                 osc_advance_fraction_of_wave(sh, -(1.0 / (2.0 * M_PI)) * st_err * 0.05);
                 osc_set_phase_deg(st, (360.0 * sh.ptr / ((double)WTSIZE)) + (360.0 * (1.0 - p.ee)));
             }
-            sig2 = cmul(sig2, savrot);                                    // :628-630
-            rot = cmul(rot, make_double2(cos(rot_freq), sin(rot_freq)));
-            sig2 = cmul(sig2, rot);
+            sig2 = c_mul(sig2, savrot);                                    // :628-630
+            rot = c_mul(rot, make_double2(cos(rot_freq), sin(rot_freq)));
+            sig2 = c_mul(sig2, rot);
             {   // MSKEbNoMeasure::Update(std::abs(sig2)) (DSP.cpp:493-505)
                 const double ab = hypot(sig2.x, sig2.y), sq = ab * ab;
                 const size_t e = (size_t)eb_pos * cp + ch;
@@ -643,7 +532,7 @@ burst_back_kernel(const __grid_constant__ BurstParams p, int n)
                 d8_pos++; if (d8_pos >= d8_len) d8_pos = 0;
             }
             const int ts = osc_index(st.ptr);
-            const double2 st_out = cmul(make_double2(p.cos_t[ts], p.sin_t[ts]), make_double2(st_eta, -d8out));
+            const double2 st_out = c_mul(make_double2(p.cos_t[ts], p.sin_t[ts]), make_double2(st_eta, -d8out));
             const double st_angle_error = atan2_fast(st_out.y, st_out.x);
             if (cntr > p.end_rotation) osc_advance_fraction_of_wave(st, -st_angle_error * 0.002 / 360.0);   // :661-665
             double frac;
@@ -657,7 +546,7 @@ burst_back_kernel(const __grid_constant__ BurstParams p, int n)
                 if (ct_ec < -M_PI_2) ct_ec = -M_PI_2;
                 if (cntr > (p.start_processing * sps)) {                  // :680-687
                     const double ang = (1.0 * ct_ec) * 0.25;
-                    rot = cmul(rot, make_double2(cos(ang), sin(ang)));
+                    rot = c_mul(rot, make_double2(cos(ang), sin(ang)));
                     if (cntr > p.end_rotation) rot_freq = rot_freq + ct_ec * 0.0001;
                 }
                 if (cntr > (p.start_processing * sps)) {                  // :706-711 msema MA(75)
@@ -778,10 +667,10 @@ burst_oqpsk_back_kernel(const __grid_constant__ BurstParams p, long long sample0
         if ((cntr > ((256 - 10) * SPS)) && insertpreamble) { push(-1); insertpreamble = 0; }   // :531-535
         if ((cntr > SPS * (128 + 10)) && (cntr < ((256 - 10) * SPS))) {  // :538-558
             const double progress = (((double)cntr) - (SPS * (128 + 10))) / (((256 - 10) * SPS) - (SPS * (128 + 10)));
-            double2 spt = cmul(cmul(sig2, strot), make_double2(0.0, 1.0));
+            double2 spt = c_mul(c_mul(sig2, strot), make_double2(0.0, 1.0));
             const double er = tanh(spt.y) * (spt.x);
             const double ang = (1.0 * er) * 0.01;
-            strot = cmul(strot, make_double2(cos(ang), sin(ang)));
+            strot = c_mul(strot, make_double2(cos(ang), sin(ang)));
             savrot = make_double2(savrot.x * 0.95 + 0.05 * strot.x, savrot.y * 0.95 + 0.05 * strot.y);
             double a1out;
             {
@@ -794,15 +683,15 @@ burst_oqpsk_back_kernel(const __grid_constant__ BurstParams p, long long sample0
             }
             spt = make_double2(spt.x, a1out);
             const int tq = osc_index(sq.ptr);
-            const double2 q = cmul(make_double2(p.cos_t[tq], p.sin_t[tq]), make_double2(spt.x, -spt.y));
+            const double2 q = c_mul(make_double2(p.cos_t[tq], p.sin_t[tq]), make_double2(spt.x, -spt.y));
             double st_err = atan2(q.y, q.x);
             st_err *= 1.5 * (1.0 - progress * progress);
             osc_advance_fraction_of_wave(sq, -(1.0 / (2.0 * M_PI)) * st_err * 0.1);
             osc_set_phase_deg(st, ((360.0 * sq.ptr / ((double)WTSIZE))) * 4.0 + (360.0 * p.ee));
         }
-        sig2 = cmul(sig2, savrot);                                        // :562-565
-        rot = cmul(rot, make_double2(cos(rot_freq), sin(rot_freq)));
-        sig2 = cmul(sig2, rot);
+        sig2 = c_mul(sig2, savrot);                                        // :562-565
+        rot = c_mul(rot, make_double2(cos(rot_freq), sin(rot_freq)));
+        sig2 = c_mul(sig2, rot);
         const double sig2abs = hypot(sig2.x, sig2.y);
         {   // OQPSKEbNoMeasure::Update (DSP.cpp:729-744)
             const size_t e = (size_t)eb_pos * cp + ch;
@@ -852,7 +741,7 @@ burst_oqpsk_back_kernel(const __grid_constant__ BurstParams p, long long sample0
         { const double older = (p.k8 == 3) ? d8_2 : (p.k8 == 2 ? d8_1 : d8_0), newer = (p.k8 == 3) ? d8_1 : (p.k8 == 2 ? d8_0 : st_eta);
           d8out = (w8 * newer + (1.0 - w8) * older); d8_2 = d8_1; d8_1 = d8_0; d8_0 = st_eta; }
         const int ts = osc_index(st.ptr);
-        const double2 st_out = cmul(make_double2(p.cos_t[ts], p.sin_t[ts]), make_double2(st_eta, -d8out));
+        const double2 st_out = c_mul(make_double2(p.cos_t[ts], p.sin_t[ts]), make_double2(st_eta, -d8out));
         const double st_angle_error = atan2_fast(st_out.y, st_out.x);
         if (cntr > SPS * (128 + 64)) {
             osc_set_freq(st, (-st_angle_error * 0.00000001) + st.freq, p.Fs);
@@ -881,7 +770,7 @@ burst_oqpsk_back_kernel(const __grid_constant__ BurstParams p, long long sample0
                 if (ct_ec < -M_PI_2) ct_ec = -M_PI_2;
                 if (cntr > ((128 + 10) * SPS)) {                          // :641-645
                     const double ang = (1.0 * ct_ec) * 0.1;
-                    rot = cmul(rot, make_double2(cos(ang), sin(ang)));
+                    rot = c_mul(rot, make_double2(cos(ang), sin(ang)));
                     rot_freq = rot_freq + ct_ec * 0.0001;
                 }
                 if (cntr > ((128 + 10) * SPS)) {                          // :684-689 msema MA(128)
@@ -928,17 +817,9 @@ burst_oqpsk_back_kernel(const __grid_constant__ BurstParams p, long long sample0
 }
 
 // ------------------------------------------------------------------------------------------------ launches
-int hilbert_exchange_launch(const HilbertStream &h, const BurstParams &p, const int16_t *pcm, size_t stride, int pcm0, int i0, int i1, int fill0, cudaStream_t s)
+int hilbert_exchange_launch(const FastFir &h, const BurstParams &p, const int16_t *pcm, size_t stride, int pcm0, int i0, int i1, int fill0, cudaStream_t s)
 {
     hilbert_exchange_kernel<<<(p.n_channels + 63) / 64, 64, 0, s>>>(h, p, pcm, stride, pcm0, i0, i1, fill0);
-    JB_CUDA(cudaGetLastError());
-    return 0;
-}
-int hilbert_block_launch(const HilbertStream &h, int n_channels, int first_block, cudaStream_t s)
-{
-    const size_t smem = (size_t)h.nfft * sizeof(double2);
-    JB_CUDA(cudaFuncSetAttribute(hilbert_block_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    hilbert_block_kernel<<<n_channels, 1024, smem, s>>>(h, first_block);
     JB_CUDA(cudaGetLastError());
     return 0;
 }

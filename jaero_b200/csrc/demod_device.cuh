@@ -6,6 +6,7 @@
 #pragma once
 #include "demod.cuh"
 #include "common.cuh"
+#include "fft_device.cuh"                  // c_mul
 
 namespace jb {
 
@@ -160,12 +161,6 @@ __device__ __forceinline__ double biquad_update(Biquad &q, double sig, double a1
     q.x2 = q.x1; q.x1 = sig;
     q.y2 = q.y1; q.y1 = y;
     return y;
-}
-
-// complex helpers with std::complex<double>'s evaluation order (no FMA contraction)
-__device__ __forceinline__ double2 cmul(double2 a, double2 b)
-{
-    return make_double2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x);
 }
 
 // qRound (Qt5 qglobal.h) as used at oqpskdemodulator.cpp:569 / mskdemodulator.cpp:453

@@ -250,7 +250,7 @@ __device__ __forceinline__ void oqpsk_symbol_tail(const DemodParams &p, int ch, 
         t.dt_pos++; if (t.dt_pos >= p.dt_len) t.dt_pos = 0;
         pt_qpsk = t.dt_old;
     }
-    pt_qpsk = cmul(pt_qpsk, make_double2(cos(t.marg_val), sin(t.marg_val)));   // :537
+    pt_qpsk = c_mul(pt_qpsk, make_double2(cos(t.marg_val), sin(t.marg_val)));   // :537
     t.sc1 = t.sc0; t.sc0 = pt_qpsk;                                              // pointbuff (:546), decimated
     {   // MSEcalc::Update (DSP.cpp:451-463)
         const size_t e = (size_t)t.mse_pos * p.cpad + ch;
@@ -325,7 +325,7 @@ __device__ __forceinline__ void msk_symbol_tail(const DemodParams &p, int ch, bo
         t.dt_pos++; t.dt_pos %= p.dt_len;
         pt_msk = p.dt_ring[(size_t)t.dt_pos * p.cpad + ch];
     }
-    pt_msk = cmul(pt_msk, make_double2(cos(t.marg_val), sin(t.marg_val)));            // :431
+    pt_msk = c_mul(pt_msk, make_double2(cos(t.marg_val), sin(t.marg_val)));            // :431
     t.sc1 = t.sc0; t.sc0 = make_double2(pt_msk.x * 0.75, pt_msk.y * 0.75);           // pointbuff (:440)
     {   // :446-448
         const double tda = (fabs((pt_msk).x * 0.75) - 1.0), tdb = (fabs((pt_msk).y * 0.75) - 1.0);

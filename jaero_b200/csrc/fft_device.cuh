@@ -1,11 +1,15 @@
-// Double-precision complex FFT building blocks shared by the coarse estimator (cfe.cu) and the wideband scanner (scan.cu).
-// Stockham autosort passes with radix-8 / radix-4 butterflies kept in registers over TILE independent sequences held in natural
-// order in shared memory rows s[f][.] (row pitch LD).
+// Double-precision complex arithmetic and FFT building blocks: the complex helpers and butterflies of every device FFT (coarse
+// estimator, wideband scanner, FFT convolution, trident FFTs) and the demodulators' complex products, plus the Stockham autosort
+// pass with radix-8 / radix-4 butterflies kept in registers over TILE independent sequences held in natural order in shared
+// memory rows s[f][.] (row pitch LD) that the estimator and the scanner use.
 #pragma once
 #include <cuda_runtime.h>
 
 namespace jb {
 
+// Written in std::complex<double>'s evaluation order. Whether the products and sums contract into FMAs is decided by the flags of
+// the translation unit that inlines them: prefilter.cu, fastfir.cu, burst.cu and demod_kernels.cu are built with -fmad=false,
+// so that they round as the CPU reference does (x86-64 has no implicit FMA contraction); cfe.cu and scan.cu let them contract.
 __device__ __forceinline__ double2 c_add(double2 a, double2 b) { return make_double2(a.x + b.x, a.y + b.y); }
 __device__ __forceinline__ double2 c_sub(double2 a, double2 b) { return make_double2(a.x - b.x, a.y - b.y); }
 __device__ __forceinline__ double2 c_mul(double2 a, double2 b) { return make_double2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }

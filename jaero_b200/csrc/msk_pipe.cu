@@ -264,7 +264,7 @@ msk_pipe_kernel(const __grid_constant__ DemodParams p, const SegmentArgs a, cons
             const double dnxt = (i + 1 < a.i1) ? in.dval(i + 1) : 0.0;
             nb_sync(MB_YT + sl);                               // st_eta, d8out of this sample (warp E)
             const double st_eta = HAND(sl, 6), d8out = HAND(sl, 7);
-            const double2 st_out = cmul(make_double2(cs_re, cs_im), make_double2(st_eta, -d8out));   // :389-390
+            const double2 st_out = c_mul(make_double2(cs_re, cs_im), make_double2(st_eta, -d8out));   // :389-390
             const double st_angle_error = atan2_fast(st_out.y, st_out.x);                          // :392
             const double weighting = fabs(tanh(st_angle_error));                              // :395
             osc_advance_fraction_of_wave(st, -(1.0 - weighting) * st_angle_error * gain);

@@ -245,7 +245,7 @@ oqpsk_segment_kernel(const __grid_constant__ DemodParams p, const SegmentArgs a,
             // sig2 = mixer2.WTCISValue()*cval_prefiltered[i] (:440); mixer2_freq_sum+=mixer2.GetFreqHz() (:447)
             double2 xv = *reinterpret_cast<const double2 *>(t_x + (pt & 1) * OQ_SM_X + lane * OQ_XROW + po * 16);
             if (!live) xv = make_double2(0.0, 0.0);
-            const double2 sg = cmul(make_double2(c2_re, c2_im), xv);
+            const double2 sg = c_mul(make_double2(c2_re, c2_im), xv);
             fre = sg.x; fim = sg.y;
             m2sum += m2.freq;
         }
@@ -302,7 +302,7 @@ oqpsk_segment_kernel(const __grid_constant__ DemodParams p, const SegmentArgs a,
             d8out = (w8 * newer + (1.0 - w8) * older);
             d8_2 = d8_1; d8_1 = d8_0; d8_0 = st_eta;
         }
-        const double2 st_out = cmul(make_double2(cs_re, cs_im), make_double2(st_eta, -d8out));   // :478-479
+        const double2 st_out = c_mul(make_double2(cs_re, cs_im), make_double2(st_eta, -d8out));   // :478-479
         const double st_angle_error = atan2_fast(st_out.y, st_out.x);          // :480 std::arg
         osc_set_freq(st, (-st_angle_error * 0.00000001) + st.freq, Fs);   // :481 IncreseFreqHz
         osc_advance_fraction_of_wave(st, -st_angle_error * 0.01 / 360.0); // :482

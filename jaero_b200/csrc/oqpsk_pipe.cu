@@ -237,7 +237,7 @@ oqpsk_pipe_kernel(const __grid_constant__ DemodParams p, const SegmentArgs a, co
             const double ns_re = cos_t[st_spec], ns_im = sin_t[st_spec];
             nb_sync(BAR_YT + sl);                              // st_eta, d8out of this sample (warp E)
             const double st_eta = HAND(sl, 4), d8out = HAND(sl, 5);
-            const double2 st_out = cmul(make_double2(cs_re, cs_im), make_double2(st_eta, -d8out));   // :478-479
+            const double2 st_out = c_mul(make_double2(cs_re, cs_im), make_double2(st_eta, -d8out));   // :478-479
             const double st_angle_error = atan2_fast(st_out.y, st_out.x);     // :480 std::arg
             osc_set_freq(st, (-st_angle_error * 0.00000001) + st.freq, Fs);   // :481 IncreseFreqHz
             osc_advance_fraction_of_wave(st, div_exact(-st_angle_error * 0.01, 360.0, 1.0 / 360.0)); // :482

@@ -1,16 +1,8 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>
+#include "fastfir.cuh"
 namespace jb {
-
-static const int FIR_L = 2048;            // block length L = nfft - K + 1 for K = 2049 taps, nfft = 4096
-
-// streaming FFT convolution state (JFastFir), channel-major so one CTA owns one channel's block
-struct FirStream {
-    double2 *H;                           // FFT4096 of the zero-padded kernel (shared by all channels)
-    double2 *tw;                          // W_4096^k
-    double2 *hist, *inblk, *outblk;       // [ch][FIR_L]
-};
 
 struct PreParams {                        // 8400 bps pre-filter front end
     int n_channels, cpad;
@@ -21,7 +13,6 @@ struct PreParams {                        // 8400 bps pre-filter front end
 };
 
 int pre_down_launch(const PreParams &q, const int16_t *pcm, size_t stride, int n, cudaStream_t s);
-int fir_exchange_up_launch(const PreParams &q, const FirStream &f, int i0, int i1, int fill0, cudaStream_t s);
-int fir_block_launch(const FirStream &f, int n_channels, int first_block, cudaStream_t s);
+int fir_exchange_up_launch(const PreParams &q, const FastFir &f, int i0, int i1, int fill0, cudaStream_t s);
 int pre_finish_launch(const PreParams &q, const double *m2_freq_sum, int n, double Fs, cudaStream_t s);
 }
