@@ -188,11 +188,7 @@ msk_pipe_kernel(const __grid_constant__ DemodParams p, const SegmentArgs a, cons
                 const double strobe = HAND(sl, 8), dnext = HAND(sl, 9);
                 double sy_flag = 0.0, sy_ec = 0.0;
                 if (strobe != 0.0) {                                              // :408
-                    const double ct_xt = tanh(sig2.y) * sig2.x;
-                    const double ct_xt_d = tanh(pt_d.x) * pt_d.y;
-                    double ct_ec = ct_xt_d - ct_xt;
-                    if (ct_ec > M_PI) ct_ec = M_PI;
-                    if (ct_ec < -M_PI) ct_ec = -M_PI;
+                    double ct_ec = ct_error(sig2, pt_d);
                     if (ct_ec > M_PI_2) ct_ec = M_PI_2;
                     if (ct_ec < -M_PI_2) ct_ec = -M_PI_2;
                     osc_increase_phase_deg(m2, aggr * 1.0 * ct_ec);

@@ -259,14 +259,13 @@ oqpsk_segment_kernel(const __grid_constant__ DemodParams p, const SegmentArgs a,
             const double sq = dabval * dabval;
             ma_push(eb_sum2, t_e2[rslot], sq);
             ma_push(eb_sum1, t_e1[rslot], dabval);
-            if (i >= eb_from) oqpsk_ebno_readout(p, eb_ebno, eb_sum1, eb_sum2);
+            if (i >= eb_from) oqpsk_ebno_readout(p.ebno_len, p.Fs, p.fb, eb_ebno, eb_sum1, eb_sum2);
         }
 
         {   // AGC::Update (DSP.cpp:370-379)
             ma_push(agc_sum, t_agc[rslot], dabval);
             ring_dirty = true;
-            agc_val = 1.414213562 / fmax(agc_sum / ((double)agc_len), 0.000001);
-            agc_val = fmax(agc_val, 0.000001);
+            agc_val = agc_gain(MeanDiv(agc_len), agc_sum);
         }
         double2 sig2 = make_double2(sre * agc_val, sim * agc_val);        // :466
         const double abval = hypot(sig2.x, sig2.y);                       // :469 std::abs
@@ -318,11 +317,7 @@ oqpsk_segment_kernel(const __grid_constant__ DemodParams p, const SegmentArgs a,
             if (!yui) pt_d = pt;
             else {
                 double2 pt_qpsk = make_double2(pt.x, pt_d.y);             // :503
-                const double ct_xt = tanh(pt.y) * pt.x;
-                const double ct_xt_d = tanh(pt_d.x) * pt_d.y;
-                double ct_ec = ct_xt_d - ct_xt;
-                if (ct_ec > M_PI) ct_ec = M_PI;
-                if (ct_ec < -M_PI) ct_ec = -M_PI;
+                double ct_ec = ct_error(pt, pt_d);
                 if (fbr > 8400) {                                         // :518-525
                     ct_ec = biquad_update(lf, ct_ec, p.lf_a1, p.lf_a2, p.lf_b0, p.lf_b1, p.lf_b2);
                     if (ct_ec > M_PI_2) ct_ec = M_PI_2;

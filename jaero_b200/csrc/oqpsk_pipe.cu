@@ -330,7 +330,7 @@ oqpsk_pipe_kernel(const __grid_constant__ DemodParams p, const SegmentArgs a, co
                     const double sq = dabval * dabval;
                     ma_push(eb_sum2, t_e2[rslot], sq);
                     ma_push(eb_sum1, t_e1[rslot], dabval);
-                    if (j >= eb_from_j) oqpsk_ebno_readout(p, eb_ebno, eb_sum1, eb_sum2);
+                    if (j >= eb_from_j) oqpsk_ebno_readout(p.ebno_len, p.Fs, p.fb, eb_ebno, eb_sum1, eb_sum2);
                 }
                 {   // AGC::Update (DSP.cpp:370-379)
                     ma_push(agc_sum, t_agc[rslot], dabval);

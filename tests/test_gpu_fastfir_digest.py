@@ -1,7 +1,9 @@
-"""GPU test (pytest -m gpu): the streaming FFT convolutions behind the 8400 bps pre-filter and the burst Hilbert filter give, bit
-for bit, the soft bits and full per-channel status recorded in tests/golden/fastfir_digests.json (tools/make_fastfir_digests.py):
-8400 bps OQPSK under writes that cut the 2048-sample pre-filter blocks at every edge, and the three burst modes on streams whose
-fills complete at and one sample after a 6145-sample Hilbert block boundary."""
+"""GPU test (pytest -m gpu): the streaming FFT convolutions behind the 8400 bps pre-filter and the burst Hilbert filter, and the
+burst demodulators behind them, give, bit for bit, the soft bits and full per-channel status recorded in
+tests/golden/fastfir_digests.json (tools/make_fastfir_digests.py): 8400 bps OQPSK under writes that cut the 2048-sample
+pre-filter blocks at every edge, the three burst modes on streams whose fills complete at and one sample after a 6145-sample
+Hilbert block boundary, and the three burst modes on every burst edge stream at once (with AFC off for MSK 1200 and the
+squelch on for burst OQPSK as well)."""
 import importlib.util
 import json
 import os

@@ -1,6 +1,6 @@
-"""SHA-256 digests of what the two streaming FFT convolutions feed: the 8400 bps pre-filter (K6, nfft 4096, 2049 taps) and the
-burst demodulators' Hilbert filter (nfft 8192, 2048 taps), seen through the C ABI as every soft bit and the full status of every
-channel (all doubles bit for bit, all ints).
+"""SHA-256 digests of what the two streaming FFT convolutions feed, the 8400 bps pre-filter (K6, nfft 4096, 2049 taps) and the
+burst demodulators' Hilbert filter (nfft 8192, 2048 taps), and of the burst demodulators' whole output, seen through the C ABI
+as every soft bit and the full status of every channel (all doubles bit for bit, all ints).
 
     python tools/make_fastfir_digests.py        # writes tests/golden/fastfir_digests.json (needs a GPU)
 
@@ -8,7 +8,10 @@ channel (all doubles bit for bit, all ints).
 under write patterns that cut the 2048-sample K6 blocks at every edge. K6's mix-up frequency is set at the end of every write
 (mixer_fir_pre.SetFreq(mixer2_freq_sum/i)), so the 8400 bps output depends on how the stream is cut and every pattern has its
 own digest. The burst modes run the tests/burst_edge_streams.py streams whose accepted fill completes at a multiple of the
-6145-sample Hilbert block and one sample after it, with 4800-sample and with odd-sized writes.
+6145-sample Hilbert block and one sample after it, with 4800-sample and with odd-sized writes. The burst_* cases pin the burst
+demodulators themselves: one channel per tests/burst_edge_streams.py stream of the mode (9 for MSK, 10 for burst OQPSK, so the
+last 32-channel group of the demodulator tail has idle lanes) under both write patterns, plus burst MSK 1200 with AFC off and
+burst OQPSK with the squelch on.
 tests/test_gpu_fastfir_digest.py recomputes the digests and compares them."""
 import hashlib
 import json
@@ -35,6 +38,8 @@ PATTERNS_8400 = {
 BURST_MODES = ["msk1200", "msk600", "oqpsk"]
 BURST_STREAMS = ["hil_edge", "hil_edge1"]
 BURST_PATTERNS = ["P1", "P2"]
+# burst_<mode>_<set>_<pattern>: "all" is every stream of the mode; "afc0" is that with AFC off, "sql" with the squelch on
+BURST_SETS = [(m, "all", p) for m in BURST_MODES for p in BURST_PATTERNS] + [("msk1200", "afc0", "P1"), ("oqpsk", "sql", "P1")]
 
 
 def _writes(pattern, n):
@@ -71,7 +76,8 @@ def _run(batch, pcm2, writes):
 
 
 def cases():
-    return ["8400_" + p for p in PATTERNS_8400] + ["%s_%s" % (m, p) for m in BURST_MODES for p in BURST_PATTERNS]
+    return (["8400_" + p for p in PATTERNS_8400] + ["%s_%s" % (m, p) for m in BURST_MODES for p in BURST_PATTERNS]
+            + ["burst_%s_%s_%s" % s for s in BURST_SETS])
 
 
 def run_case(name):
@@ -85,11 +91,20 @@ def run_case(name):
                                   signalthreshold=0.65, afc=True)
         return _run(b, pcm2, _writes(PATTERNS_8400[name[5:]], pcm2.shape[1]))
     import burst_edge_streams as S
-    mode, pattern = name.rsplit("_", 1)
+    if name.startswith("burst_"):
+        mode, streams, pattern = name[6:].split("_")
+    else:
+        (mode, pattern), streams = name.rsplit("_", 1), "edges"
     v = S.variants(mode)
-    pcm2 = np.stack([v[k] for k in BURST_STREAMS])
+    pcm2 = np.stack([v[k] for k in (BURST_STREAMS if streams == "edges" else v)])
     m = S.MODES[mode]
-    b = jaero_b200.BurstOqpskBatch(2, **m["kw"]) if m["kind"] == "burst_oqpsk" else jaero_b200.BurstMskBatch(2, **m["kw"])
+    C = pcm2.shape[0]
+    if m["kind"] == "burst_oqpsk":
+        b = jaero_b200.BurstOqpskBatch(C, sql=streams == "sql", **m["kw"])
+    else:
+        b = jaero_b200.BurstMskBatch(C, **m["kw"])
+        if streams == "afc0":
+            jaero_b200._check(jaero_b200.lib().jaero_burst_set_afc(b.h, 0))
     return _run(b, pcm2, S.cycle_writes(getattr(S, pattern), pcm2.shape[1]))
 
 
