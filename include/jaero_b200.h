@@ -163,6 +163,14 @@ int jaero_batch_cfe_geometry(const jaero_batch *b, int32_t out[6]);
  * batch is in the state an estimator epoch of jaero_batch_write leaves it in, with the caller's ring as its baseband ring. */
 int jaero_batch_probe_cfe(jaero_batch *b, const double *ring, int oldest, const int32_t *bigchange, int impl, int max_clusters,
                           int max_group, double *y_out, double *raw_est, double *emitted_est);
+/* The streaming overlap-save FFT convolution of the 8400 bps pre-filter and the burst Hilbert filter (JFastFir: per channel,
+ * y[n] = sum_k taps[k] x[n-L-k] for n >= 2L and 0 before, L = nfft - K + 1) on caller data, through the production host path and
+ * block kernel, so a test can compare it with an independent reference. taps [K] complex, x and y [n_channels][n] complex
+ * (interleaved re/im). writes[0 .. n_writes) is the sequence of write calls the samples arrive in; each must be > 0 and they
+ * must add up to n. (K, nfft) must be a pair the library has a block kernel for: (2049, 4096) or (2048, 8192). Allocates and
+ * frees its own buffers and stream on `device`. */
+int jaero_probe_fastfir(int device, int nfft, const double *taps, int K, int n_channels, const double *x, size_t n,
+                        const int32_t *writes, int n_writes, double *y);
 
 /* ---- K=7 r=1/2 soft Viterbi (polys 109,79), one independent decoder per channel ---- */
 int jaero_viterbi_create(int n_channels, int paddinglength, int device_ordinal, jaero_viterbi **out);
@@ -249,6 +257,19 @@ int jaero_burst_set_sql(jaero_burst *b, int state);
 int jaero_burst_get_status_all(jaero_burst *b, jaero_burst_status *out);
 int jaero_burst_sync(jaero_burst *b);
 int64_t jaero_burst_launch_count(const jaero_burst *b);
+/* ---- test support (not part of the drop-in surface): the trident FFTs and peak searches of a burst batch on caller segments.
+ * geometry: out = {tri_sz (samples of a fill), base_len, top_len (samples of the base / top section), nfft of the transforms}. */
+int jaero_burst_trident_geometry(const jaero_burst *b, int32_t out[4]);
+/* Writes segments[e][0 .. tri_sz) into trident slot ev_slot[e] of channel ev_channel[e] (each pair at most once, channel in
+ * [0, n_channels), slot in [0, 8)), records the events in the event table as the front kernel would, and runs the trident
+ * kernels in rounds of 128 events, as jaero_burst_write does. spectra_out [n_events][2][nfft] complex (NULL: not copied)
+ * receives the base spectrum, then the top spectrum, of each event. With spectra_in (same layout) non-NULL the FFTs are
+ * skipped and only the peak search of the batch's kind runs on the caller's spectra; segments may then be NULL.
+ * result [n_events][5]: burst MSK {minvalbin, minval, maxtoppos, maxtopposhigh, arg(base[minvalbin])}, burst OQPSK
+ * {minvalbin, |base[minvalbin]|, maxvalbin, maxval, arg(base[minvalbin])}.
+ * The probe overwrites the batch's trident buffers and event table: afterwards the batch may only be destroyed. */
+int jaero_burst_probe_trident(jaero_burst *b, int n_events, const int32_t *ev_channel, const int32_t *ev_slot, const double *segments,
+                              const double *spectra_in, double *spectra_out, double *result);
 
 /* ---- R/T burst channel layer (SURVEY.md section 8(f)2) ----
  * Replaces the burst branch of AeroL::Decode (JAERO/aerol.cpp:1124-1350, :1985-2031: unique-word detection with the

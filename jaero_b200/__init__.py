@@ -61,7 +61,7 @@ EXPORTS = ["jaero_last_error", "jaero_device_count", "jaero_batch_create", "jaer
            "jaero_pchannel_lost_signal", "jaero_pchannel_write_batch", "jaero_cchannel_lost_signal", "jaero_cchannel_write_batch", "jaero_batch_wire_signal_status",
            "jaero_burst_msk_create", "jaero_burst_oqpsk_create", "jaero_burst_destroy", "jaero_burst_write", "jaero_burst_write_device",
            "jaero_burst_read_softbits", "jaero_burst_set_dcd", "jaero_burst_get_status_all", "jaero_burst_sync",
-           "jaero_burst_launch_count",
+           "jaero_burst_launch_count", "jaero_probe_fastfir", "jaero_burst_trident_geometry", "jaero_burst_probe_trident",
            "jaero_rt_create", "jaero_rt_destroy", "jaero_rt_process_softbits", "jaero_rt_process_burst", "jaero_rt_tick",
            "jaero_rt_read_packets", "jaero_rt_get_stats", "jaero_rt_launch_count", "jaero_rt_set_vector_mode",
            "jaero_cchannel_create", "jaero_cchannel_destroy", "jaero_cchannel_process_batch", "jaero_cchannel_process_softbits",
@@ -149,6 +149,9 @@ def lib():
         L.jaero_burst_get_status_all.argtypes = [vp, vp]
         L.jaero_burst_sync.argtypes = [vp]
         L.jaero_burst_launch_count.argtypes = [vp]; L.jaero_burst_launch_count.restype = ctypes.c_int64
+        L.jaero_probe_fastfir.argtypes = [i, i, vp, i, i, vp, sz, vp, i, vp]
+        L.jaero_burst_trident_geometry.argtypes = [vp, vp]
+        L.jaero_burst_probe_trident.argtypes = [vp, i, vp, vp, vp, vp, vp, vp]
         L.jaero_rt_create.argtypes = [ctypes.c_double, i, i, ctypes.POINTER(vp)]
         L.jaero_rt_destroy.argtypes = [vp]; L.jaero_rt_destroy.restype = None
         L.jaero_rt_process_softbits.argtypes = [vp, vp, sz, vp]
@@ -210,6 +213,18 @@ def _check(rc):
 
 def _p(a):
     return a.ctypes.data_as(ctypes.c_void_p)
+
+
+def probe_fastfir(taps, x, nfft, writes, device=0):
+    """test support: the streaming FFT convolution (include/jaero_b200.h, jaero_probe_fastfir) of x [n_channels, n] complex with
+    taps [K] complex, fed as the write calls `writes` (sizes adding up to n). -> y [n_channels, n] complex"""
+    h = np.ascontiguousarray(taps, dtype=np.complex128)
+    x = np.ascontiguousarray(x, dtype=np.complex128)
+    assert h.ndim == 1 and x.ndim == 2
+    w = np.ascontiguousarray(writes, dtype=np.int32)
+    y = np.zeros_like(x)
+    _check(lib().jaero_probe_fastfir(int(device), int(nfft), _p(h), len(h), x.shape[0], _p(x), x.shape[1], _p(w), len(w), _p(y)))
+    return y
 
 
 class DemodBatch:
@@ -521,6 +536,31 @@ class BurstMskBatch:
 
     def sync(self):
         _check(lib().jaero_burst_sync(self.h))
+
+    def trident_geometry(self):
+        """test support: dict(tri_sz, base_len, top_len, nfft) of the trident test"""
+        o = np.zeros(4, dtype=np.int32)
+        _check(lib().jaero_burst_trident_geometry(self.h, _p(o)))
+        return dict(zip(("tri_sz", "base_len", "top_len", "nfft"), (int(v) for v in o)))
+
+    def probe_trident(self, channels, slots, segments=None, spectra_in=None, want_spectra=False):
+        """test support: the trident kernels on segments [n, tri_sz] placed in (channel, slot) fills (include/jaero_b200.h,
+        jaero_burst_probe_trident); spectra_in [n, 2, nfft] complex runs only the peak search. Overwrites the batch's trident
+        state: afterwards the batch may only be closed. -> (result [n, 5], spectra [n, 2, nfft] complex or None)"""
+        g = self.trident_geometry()
+        ch = np.ascontiguousarray(channels, dtype=np.int32)
+        sl = np.ascontiguousarray(slots, dtype=np.int32)
+        n = len(ch)
+        assert sl.shape == (n,)
+        seg = None if segments is None else np.ascontiguousarray(segments, dtype=np.float64)
+        assert seg is None or seg.shape == (n, g["tri_sz"])
+        sin = None if spectra_in is None else np.ascontiguousarray(spectra_in, dtype=np.complex128)
+        assert sin is None or sin.shape == (n, 2, g["nfft"])
+        res = np.zeros((n, 5), dtype=np.float64)
+        sout = np.zeros((n, 2, g["nfft"]), dtype=np.complex128) if want_spectra else None
+        _check(lib().jaero_burst_probe_trident(self.h, n, _p(ch), _p(sl), None if seg is None else _p(seg),
+                                               None if sin is None else _p(sin), None if sout is None else _p(sout), _p(res)))
+        return res, sout
 
     @property
     def launches(self):

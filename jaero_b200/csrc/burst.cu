@@ -812,6 +812,10 @@ int burst_trident_fft_launch(const BurstParams &p, const int *d_ev_list, int n_e
 {
     trident_fft_kernel<<<2 * n_events, 1024, 0, s>>>(p, d_ev_list, n_events, wa, wb, tw);
     JB_CUDA(cudaGetLastError());
+    return burst_trident_peaks_launch(p, d_ev_list, n_events, wa, wb, s);
+}
+int burst_trident_peaks_launch(const BurstParams &p, const int *d_ev_list, int n_events, double2 *wa, const double2 *wb, cudaStream_t s)
+{
     if (p.kind == 1) trident_peaks_oqpsk_kernel<<<n_events, 1024, 0, s>>>(p, d_ev_list, n_events, wb, wa);
     else trident_peaks_kernel<<<n_events, 1024, 0, s>>>(p, d_ev_list, n_events, wb);
     JB_CUDA(cudaGetLastError());

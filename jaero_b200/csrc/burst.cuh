@@ -75,6 +75,8 @@ int hilbert_exchange_launch(const FastFir &h, const BurstParams &p, const int16_
 int burst_front_launch(const BurstParams &p, long long sample0, int n, cudaStream_t s);
 // trident FFTs and peak search of n_events fills; d_ev_list holds (channel, event) pairs
 int burst_trident_fft_launch(const BurstParams &p, const int *d_ev_list, int n_events, double2 *wa, double2 *wb, const double2 *tw, cudaStream_t s);
+// only the peak search of the object's kind, on the spectra already in wb (base 2e, top 2e+1); burst OQPSK uses wa as scratch
+int burst_trident_peaks_launch(const BurstParams &p, const int *d_ev_list, int n_events, double2 *wa, const double2 *wb, cudaStream_t s);
 int burst_back_launch(const BurstParams &p, long long sample0, int n, int new_write, cudaStream_t s);
 
 } // namespace jb

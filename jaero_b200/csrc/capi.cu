@@ -891,6 +891,66 @@ int jaero_batch_probe_cfe(jaero_batch *b, const double *ring, int oldest, const 
     return JAERO_OK;
 }
 
+} // extern "C"
+
+// ---- test support: the streaming FFT convolution on caller data (not part of the drop-in surface)
+namespace {
+struct FirProbe {
+    int device; cudaStream_t stream;
+    std::vector<void *> allocs;
+};
+void fir_probe_destroy(FirProbe *o)
+{
+    cudaSetDevice(o->device);
+    if (o->stream) cudaStreamSynchronize(o->stream);
+    release(o, {}, {}, o->stream);
+}
+} // namespace
+
+extern "C" {
+
+int jaero_probe_fastfir(int device, int nfft, const double *taps, int K, int n_channels, const double *x, size_t n,
+                        const int32_t *writes, int n_writes, double *y)
+{
+    if (!taps || !x || !writes || !y || n_channels <= 0 || n_writes <= 0 || n == 0 || n > 0x7fffffff) {
+        set_error("jaero_probe_fastfir: null argument or bad n_channels / n / n_writes"); return JAERO_E_ARG; }
+    if (!fastfir_size_supported(K, nfft)) {
+        set_error("jaero_probe_fastfir: no FFT convolution kernel for " + std::to_string(K) + " taps at nfft " + std::to_string(nfft));
+        return JAERO_E_ARG;
+    }
+    long long total = 0;
+    for (int w = 0; w < n_writes; w++) {
+        if (writes[w] <= 0) { set_error("jaero_probe_fastfir: write " + std::to_string(w) + " has size <= 0"); return JAERO_E_ARG; }
+        total += writes[w];
+    }
+    if (total != (long long)n) {
+        set_error("jaero_probe_fastfir: the write sizes add up to " + std::to_string(total) + ", not n = " + std::to_string(n));
+        return JAERO_E_ARG;
+    }
+    CreateGuard<FirProbe> guard(fir_probe_destroy);          // frees the buffers and the stream on every return
+    { int r = guard.begin("jaero_probe_fastfir", device); if (r) return r; }
+    FirProbe *o = guard.obj;
+    std::vector<std::complex<double>> h(K);
+    for (int k = 0; k < K; k++) h[k] = std::complex<double>(taps[2 * k], taps[2 * k + 1]);
+    FastFir f;
+    { int r = fastfir_create(o, h, nfft, n_channels, f); if (r) return r; }
+    const size_t C = n_channels;
+    double2 *dx = 0, *dy = 0;
+    if (owned_alloc(o, &dx, C * n) || owned_alloc(o, &dy, C * n)) return JAERO_E_CUDA;
+    JB_CUDA(cudaMemcpyAsync(dx, x, C * n * sizeof(double2), cudaMemcpyHostToDevice, o->stream));
+    long long launches = 0;
+    int pos = 0;
+    for (int w = 0; w < n_writes; w++) {                      // one fastfir_feed per write, as a filter's write call runs it
+        if (fastfir_feed(f, writes[w], n_channels, o->stream, &launches, [&](int i0, int i1, int fill0) {
+                return fastfir_probe_exchange_launch(f, n_channels, dx, dy, n, pos + i0, pos + i1, fill0, o->stream); }))
+            return JAERO_E_CUDA;
+        pos += writes[w];
+    }
+    JB_CUDA(cudaMemcpyAsync(y, dy, C * n * sizeof(double2), cudaMemcpyDeviceToHost, o->stream));
+    JB_CUDA(cudaStreamSynchronize(o->stream));
+    return JAERO_OK;
+}
+
 int jaero_batch_sync(jaero_batch *b)
 {
     if (!b) { set_error("null handle"); return JAERO_E_ARG; }
@@ -1700,6 +1760,61 @@ int jaero_burst_get_status_all(jaero_burst *b, jaero_burst_status *out)
         s.n_sig_true = I(BI_SIG_TRUE); s.n_sig_false = I(BI_SIG_FALSE); s.cntr = I(BI_CNTR); s.startstop = I(BI_STARTSTOP);
         s.last_burst_ebno = D(BD_LAST_EBNO_EMIT); s.n_ebno_emits = I(BI_EBNO_EMITS);
     }
+    return JAERO_OK;
+}
+
+// ---- test support: the trident FFTs and peak searches on caller segments (not part of the drop-in surface)
+int jaero_burst_trident_geometry(const jaero_burst *b, int32_t out[4])
+{
+    if (!b || !out) { set_error("jaero_burst_trident_geometry: null argument"); return JAERO_E_ARG; }
+    out[0] = b->p.tri_sz; out[1] = b->p.tri_nb; out[2] = b->p.tri_nt; out[3] = TRI_N;
+    return JAERO_OK;
+}
+int jaero_burst_probe_trident(jaero_burst *b, int n_events, const int32_t *ev_channel, const int32_t *ev_slot, const double *segments,
+                              const double *spectra_in, double *spectra_out, double *result)
+{
+    if (!b || n_events <= 0 || !ev_channel || !ev_slot || (!segments && !spectra_in) || !result) {
+        set_error("jaero_burst_probe_trident: null argument or n_events <= 0"); return JAERO_E_ARG; }
+    BurstParams &p = b->p;
+    const int C = p.n_channels;
+    // event e of the probe is event number ev[e] of its channel, in the order given, and its fill sits in slot ev_slot[e]:
+    // the kernels find the slot through ev_sample's slot field, as after burst_front
+    std::vector<int> ev_count(C, 0), ev_list(2 * (size_t)n_events), ev_table((size_t)C * BURST_MAXEV, 0);
+    std::vector<char> used((size_t)C * BURST_MAXEV, 0);
+    for (int e = 0; e < n_events; e++) {
+        const int ch = ev_channel[e], slot = ev_slot[e];
+        if (ch < 0 || ch >= C) { set_error("jaero_burst_probe_trident: event " + std::to_string(e) + ": channel out of range"); return JAERO_E_ARG; }
+        if (slot < 0 || slot >= BURST_MAXEV) { set_error("jaero_burst_probe_trident: event " + std::to_string(e) + ": slot outside [0, BURST_MAXEV)"); return JAERO_E_ARG; }
+        if (used[(size_t)ch * BURST_MAXEV + slot]) { set_error("jaero_burst_probe_trident: event " + std::to_string(e) + ": (channel, slot) appears twice"); return JAERO_E_ARG; }
+        used[(size_t)ch * BURST_MAXEV + slot] = 1;
+        const int ev = ev_count[ch]++;
+        ev_list[2 * e] = ch; ev_list[2 * e + 1] = ev;
+        ev_table[(size_t)ch * BURST_MAXEV + ev] = ev | (slot << 24);
+    }
+    JB_CUDA(cudaSetDevice(b->device));
+    const cudaStream_t s = b->stream;
+    JB_CUDA(cudaStreamSynchronize(s));
+    // every copy below reads host memory that stays alive until the final synchronisation
+    if (!spectra_in)
+        for (int e = 0; e < n_events; e++)
+            JB_CUDA(cudaMemcpyAsync(p.tri + ((size_t)ev_channel[e] * BURST_MAXEV + ev_slot[e]) * p.tri_sz, segments + (size_t)e * p.tri_sz,
+                                    (size_t)p.tri_sz * sizeof(double), cudaMemcpyHostToDevice, s));
+    JB_CUDA(cudaMemcpyAsync(p.ev_sample, ev_table.data(), ev_table.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+    JB_CUDA(cudaMemcpyAsync(b->d_ev_list, ev_list.data(), ev_list.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+    const size_t spec = (size_t)2 * TRI_N * 2;                         // doubles per event: base then top, complex
+    for (int e0 = 0; e0 < n_events; e0 += b->ev_round) {               // rounds as jaero_burst_write_device runs them
+        const int cnt = std::min(b->ev_round, n_events - e0);
+        if (spectra_in) {
+            JB_CUDA(cudaMemcpyAsync(b->wb, spectra_in + e0 * spec, cnt * spec * sizeof(double), cudaMemcpyHostToDevice, s));
+            if (burst_trident_peaks_launch(p, b->d_ev_list + 2 * e0, cnt, b->wa, b->wb, s)) return JAERO_E_CUDA;
+        } else if (burst_trident_fft_launch(p, b->d_ev_list + 2 * e0, cnt, b->wa, b->wb, b->tw32k, s)) return JAERO_E_CUDA;
+        if (spectra_out) JB_CUDA(cudaMemcpyAsync(spectra_out + e0 * spec, b->wb, cnt * spec * sizeof(double), cudaMemcpyDeviceToHost, s));
+    }
+    std::vector<double> res((size_t)C * BURST_MAXEV * 8);
+    JB_CUDA(cudaMemcpyAsync(res.data(), p.ev_result, res.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
+    JB_CUDA(cudaStreamSynchronize(s));
+    for (int e = 0; e < n_events; e++)
+        for (int q = 0; q < 5; q++) result[5 * e + q] = res[((size_t)ev_list[2 * e] * BURST_MAXEV + ev_list[2 * e + 1]) * 8 + q];
     return JAERO_OK;
 }
 

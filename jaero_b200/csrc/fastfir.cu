@@ -98,4 +98,30 @@ int fastfir_block_launch(const FastFir &f, int n_channels, int first_block, cuda
     return f.nfft == 4096 ? block_launch<4096, 2049>(f, n_channels, first_block, s) : block_launch<8192, 2048>(f, n_channels, first_block, s);
 }
 
+// test support (jaero_probe_fastfir): the sample exchange with no per-sample work of its own, thread per channel;
+// x and y are [ch][xstride]
+__global__ void fastfir_probe_exchange_kernel(FastFir f, int n_channels, const double2 *__restrict__ x, double2 *__restrict__ y,
+                                              size_t xstride, int i0, int i1, int fill0)
+{
+    const int ch = blockIdx.x * blockDim.x + threadIdx.x;
+    if (ch >= n_channels) return;
+    double2 *inb = f.inblk + (size_t)ch * f.L;
+    const double2 *outb = f.outblk + (size_t)ch * f.L;
+    const double2 *xr = x + (size_t)ch * xstride;
+    double2 *yr = y + (size_t)ch * xstride;
+    int fill = fill0;
+    for (int i = i0; i < i1; i++) {
+        yr[i] = outb[fill];
+        inb[fill] = xr[i];
+        fill++;
+    }
+}
+int fastfir_probe_exchange_launch(const FastFir &f, int n_channels, const double2 *x, double2 *y, size_t xstride, int i0, int i1, int fill0,
+                                  cudaStream_t s)
+{
+    fastfir_probe_exchange_kernel<<<(n_channels + 63) / 64, 64, 0, s>>>(f, n_channels, x, y, xstride, i0, i1, fill0);
+    JB_CUDA(cudaGetLastError());
+    return 0;
+}
+
 } // namespace jb

@@ -23,5 +23,8 @@ struct FastFir {
 inline bool fastfir_size_supported(int K, int nfft) { return (nfft == 4096 && K == 2049) || (nfft == 8192 && K == 2048); }
 
 int fastfir_block_launch(const FastFir &f, int n_channels, int first_block, cudaStream_t s);
+// test support: the exchange as a plain copy, y[ch][i] = outblk[fill], inblk[fill] = x[ch][i] for i in [i0, i1), fill from fill0
+int fastfir_probe_exchange_launch(const FastFir &f, int n_channels, const double2 *x, double2 *y, size_t xstride, int i0, int i1, int fill0,
+                                  cudaStream_t s);
 
 } // namespace jb

@@ -62,6 +62,27 @@ def lib():
     return _lib
 
 
+_FASTFIR_SO = os.path.join(_HERE, "_ref", "libjaero_ref_fastfir.so")
+_fastfir_lib = None
+
+
+def fastfir_available():
+    return os.path.exists(_FASTFIR_SO)
+
+
+def fastfir_lib():
+    """oracle/_ref/libjaero_ref_fastfir.so (ref_fastfir_driver.cpp): jref_jfastfir(taps_ri, K, nfft, inout_ri, n, writes,
+    n_writes) drives the reference's JFastFir piecewise; jref_hilbert_kernel(out_ri) returns QJHilbertFilter's kernel"""
+    global _fastfir_lib
+    if _fastfir_lib is None:
+        L = ctypes.CDLL(_FASTFIR_SO)
+        vp, i, l = ctypes.c_void_p, ctypes.c_int, ctypes.c_long
+        L.jref_jfastfir.argtypes = [vp, i, i, vp, l, vp, i]
+        L.jref_hilbert_kernel.argtypes = [vp]
+        _fastfir_lib = L
+    return _fastfir_lib
+
+
 def _p(a):
     return a.ctypes.data_as(ctypes.c_void_p)
 

@@ -96,10 +96,11 @@ class OracleDemod:
         n = lib().jor_cfe_log_take(self.h, _p(out), len(out), int(bool(raw)))
         return out[:n].copy()
 
-    def take_aux(self, which):
+    def take_aux(self, which, cap=1 << 14):
         """burst kinds: 0 = EbNo of each burst, 1 = trident log (5 values per test), 2 = stream index of the input sample at which
-        each trident test ran (the sample that completed the fill). Each log is drained independently."""
-        out = np.zeros(1 << 14, dtype=np.float64)
+        each trident test ran (the sample that completed the fill), 3 = the trident buffer of each test (tri_sz samples per
+        test). Each log is drained independently; at most `cap` values per call."""
+        out = np.zeros(cap, dtype=np.float64)
         n = lib().jor_aux_take(self.h, which, _p(out), len(out))
         return out[:n].copy()
 

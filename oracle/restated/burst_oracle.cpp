@@ -150,6 +150,7 @@ void BurstMskOracle::writeData(const int16_t *ptr, long numofsamples)
             bool accept = minval > 500.0 && std::abs(distfrompeak - peakspacingbins) < std::abs(peakspacingbins / 20) && !(dcd) && !(cntr > 0 && cntr < (500 * SamplesPerSymbol));
             trident_log.push_back(minvalbin); trident_log.push_back(minval); trident_log.push_back(maxtoppos); trident_log.push_back(maxtopposhigh); trident_log.push_back(accept ? 1.0 : 0.0);
             fill_log.push_back((double)(nsamp + i));
+            segment_log.insert(segment_log.end(), tridentbuffer.begin(), tridentbuffer.end());
             if (accept) {
                 vol_gain = 1.4142 * (500.0 / (minval / 3));
                 double carrierphase = std::arg(out_base[minvalbin]) - (M_PI / 4.0);
@@ -336,6 +337,7 @@ void BurstOqpskOracle::writeData(const int16_t *ptr, long numofsamples)
             bool accept = (maxval > 500.0) && (fabs((((double)(maxvalbin - minvalbin))) * hzperbin) < 20.0);
             trident_log.push_back(minvalbin); trident_log.push_back(minval); trident_log.push_back(maxvalbin); trident_log.push_back(maxval); trident_log.push_back(accept ? 1.0 : 0.0);
             fill_log.push_back((double)(nsamp + i));
+            segment_log.insert(segment_log.end(), tridentbuffer.begin(), tridentbuffer.end());
             if (accept) {
                 double carrierphase = std::arg(out_base[(int)minvalbin]) - (M_PI / 4.0);
                 mixer2.SetFreq(hzperbin * minvalbin);

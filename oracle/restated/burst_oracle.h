@@ -65,6 +65,7 @@ struct BurstMskOracle                                    // burstmskdemodulator.
     std::vector<short> soft_out; std::vector<double> ebno_log; long n_sig_true, n_sig_false;
     std::vector<double> trident_log;                   // per trident test: minvalbin, minval, maxtoppos, maxtopposhigh, accepted
     std::vector<double> fill_log;                      // per trident test: stream index of the input sample that completed the fill
+    std::vector<double> segment_log;                   // per trident test: the tridentbuffer_sz samples of the completed fill
     long nsamp;                                        // input samples consumed so far
     BurstMskOracle(double fb, double Fs, double freq_center, double lockingbw, double signalthreshold);
     void writeData(const int16_t *pcm, long n);        // :371-754
@@ -91,6 +92,7 @@ struct BurstOqpskOracle                                  // burstoqpskdemodulato
     std::vector<short> soft_out; std::vector<double> ebno_log; long n_sig_true, n_sig_false;
     std::vector<double> trident_log;                   // per trident test: minvalbin, minval, maxvalbin, maxval, accepted
     std::vector<double> fill_log;                      // per trident test: stream index of the input sample that completed the fill
+    std::vector<double> segment_log;                   // per trident test: the tridentbuffer_sz samples of the completed fill
     long nsamp;                                        // input samples consumed so far
     BurstOqpskOracle(double fb, double Fs, double freq_center, double lockingbw, double signalthreshold);
     void writeData(const int16_t *pcm, long n);        // writeDataSlot :315-737 (mono)

@@ -30,12 +30,13 @@ void jor_set_dcd(void *hv, int d)
 static std::vector<short> &soft_of(OrHandle *h) { return h->kind == 0 ? h->oq->soft_out : (h->kind == 1 ? h->msk->soft_out : (h->kind == 2 ? h->bmsk->soft_out : h->boq->soft_out)); }
 long jor_soft_count(void *hv)
 { OrHandle *h = (OrHandle *)hv; return (long)soft_of(h).size(); }
-// burst: 0 = EbNo per burst, 1 = trident log (5 values per test), 2 = stream index of the sample that completed each fill
+// burst: 0 = EbNo per burst, 1 = trident log (5 values per test), 2 = stream index of the sample that completed each fill,
+// 3 = the samples of each completed fill (tridentbuffer_sz per test)
 long jor_aux_take(void *hv, int which, double *out, long cap)
 {
-    OrHandle *h = (OrHandle *)hv; if (h->kind < 2 || which < 0 || which > 2) return 0;
-    std::vector<double> &v = h->kind == 2 ? (which == 0 ? h->bmsk->ebno_log : which == 1 ? h->bmsk->trident_log : h->bmsk->fill_log)
-                                          : (which == 0 ? h->boq->ebno_log : which == 1 ? h->boq->trident_log : h->boq->fill_log);
+    OrHandle *h = (OrHandle *)hv; if (h->kind < 2 || which < 0 || which > 3) return 0;
+    std::vector<double> &v = h->kind == 2 ? (which == 0 ? h->bmsk->ebno_log : which == 1 ? h->bmsk->trident_log : which == 2 ? h->bmsk->fill_log : h->bmsk->segment_log)
+                                          : (which == 0 ? h->boq->ebno_log : which == 1 ? h->boq->trident_log : which == 2 ? h->boq->fill_log : h->boq->segment_log);
     long n = (long)v.size(); if (n > cap) n = cap;
     memcpy(out, v.data(), n * sizeof(double)); v.erase(v.begin(), v.begin() + n); return n;
 }
