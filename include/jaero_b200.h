@@ -171,6 +171,34 @@ int jaero_batch_probe_cfe(jaero_batch *b, const double *ring, int oldest, const 
  * frees its own buffers and stream on `device`. */
 int jaero_probe_fastfir(int device, int nfft, const double *taps, int K, int n_channels, const double *x, size_t n,
                         const int32_t *writes, int n_writes, double *y);
+/* The demodulators' device arithmetic primitives (jaero_b200/csrc/demod_device.cuh, cfe.cu) on caller operands, compiled with the
+ * flags the product builds them with, so a test can compare them with exact and long-double references:
+ * out[i] = op(a[i], b[i]) for i < n; integer results are returned as doubles. b is read only by the two-operand ops (NULL
+ * otherwise). Allocates and frees its own buffers and stream on `device`. */
+#define JAERO_MATH_DIV_EXACT 0     /* div_exact(a, b, 1.0 / b): the moving-average means (demod_kernels.cu, -fmad=false) */
+#define JAERO_MATH_DIV_FAST 1      /* div_fast(a, b) as demod_kernels.cu compiles it */
+#define JAERO_MATH_ATAN2_FAST 2    /* atan2_fast(y = a, x = b) */
+#define JAERO_MATH_HYPOT_FAST 3    /* hypot_fast(a, b) */
+#define JAERO_MATH_LOG10_GE1 4     /* log10_ge1(a), a >= 1, as cfe.cu compiles it */
+#define JAERO_MATH_OSC_INDEX 5     /* osc_index(a): the WaveTable entry WTCISValue reads */
+#define JAERO_MATH_Q_ROUND 6       /* q_round(a): qRound */
+#define JAERO_MATH_FMOD360 7       /* fmod360(a): fmod(a, 360) */
+#define JAERO_MATH_DIV_FAST_CFE 8  /* div_fast(a, b) as cfe.cu compiles it */
+int jaero_probe_math(int device, int op, size_t n, const double *a, const double *b, double *out);
+/* n_lanes independent WaveTable oscillators, each running its own script of n_ops operations through the device Osc helpers:
+ * lane l's k-th operation is op[l*n_ops + k] applied with argument arg[l*n_ops + k]. Every lane starts at ptr = last = step =
+ * freq = 0 and a passing fraction of 0, with sample rate `samplerate` (an integer for JAERO_OSC_SET_FREQ_SR). After each operation log[(l*n_ops + k)*7 + f] holds
+ * f = 0 ptr, 1 last ptr, 2 step, 3 freq, 4 the table index (osc_index of ptr; for JAERO_OSC_NEXT_INDEX the index after the next
+ * frame), 5 the flag JAERO_OSC_HAVE_PASSED_POINT returned (0 for the other ops), 6 the latest passing fraction. */
+#define JAERO_OSC_SET_FREQ 0          /* osc_set_freq(arg): SetFreq(arg) */
+#define JAERO_OSC_NEXT_FRAME 1        /* osc_next_frame: WTnextFrame() */
+#define JAERO_OSC_NEXT_INDEX 2        /* osc_next_index: the index WTnextFrame() + WTCISValue() would read; the state is kept */
+#define JAERO_OSC_INCREASE_PHASE_DEG 3 /* osc_increase_phase_deg(arg): IncresePhaseDeg(arg) */
+#define JAERO_OSC_SET_PHASE_DEG 4     /* osc_set_phase_deg(arg): SetPhaseDeg(arg) */
+#define JAERO_OSC_ADVANCE_FRACTION 5  /* osc_advance_fraction_of_wave(arg): AdvanceFractionOfWave(arg) */
+#define JAERO_OSC_HAVE_PASSED_POINT 6 /* osc_have_passed_point(arg): IfHavePassedPoint(arg) */
+#define JAERO_OSC_SET_FREQ_SR 7       /* osc_set_freq_wrap(arg, (int)samplerate): SetFreq(arg, samplerate), which also wraps ptr */
+int jaero_probe_osc(int device, int n_lanes, int n_ops, const int32_t *op, const double *arg, double samplerate, double *log);
 
 /* ---- K=7 r=1/2 soft Viterbi (polys 109,79), one independent decoder per channel ---- */
 int jaero_viterbi_create(int n_channels, int paddinglength, int device_ordinal, jaero_viterbi **out);

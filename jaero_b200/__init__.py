@@ -61,7 +61,7 @@ EXPORTS = ["jaero_last_error", "jaero_device_count", "jaero_batch_create", "jaer
            "jaero_pchannel_lost_signal", "jaero_pchannel_write_batch", "jaero_cchannel_lost_signal", "jaero_cchannel_write_batch", "jaero_batch_wire_signal_status",
            "jaero_burst_msk_create", "jaero_burst_oqpsk_create", "jaero_burst_destroy", "jaero_burst_write", "jaero_burst_write_device",
            "jaero_burst_read_softbits", "jaero_burst_set_dcd", "jaero_burst_get_status_all", "jaero_burst_sync",
-           "jaero_burst_launch_count", "jaero_probe_fastfir", "jaero_burst_trident_geometry", "jaero_burst_probe_trident",
+           "jaero_burst_launch_count", "jaero_probe_fastfir", "jaero_probe_math", "jaero_probe_osc", "jaero_burst_trident_geometry", "jaero_burst_probe_trident",
            "jaero_rt_create", "jaero_rt_destroy", "jaero_rt_process_softbits", "jaero_rt_process_burst", "jaero_rt_tick",
            "jaero_rt_read_packets", "jaero_rt_get_stats", "jaero_rt_launch_count", "jaero_rt_set_vector_mode",
            "jaero_cchannel_create", "jaero_cchannel_destroy", "jaero_cchannel_process_batch", "jaero_cchannel_process_softbits",
@@ -150,6 +150,8 @@ def lib():
         L.jaero_burst_sync.argtypes = [vp]
         L.jaero_burst_launch_count.argtypes = [vp]; L.jaero_burst_launch_count.restype = ctypes.c_int64
         L.jaero_probe_fastfir.argtypes = [i, i, vp, i, i, vp, sz, vp, i, vp]
+        L.jaero_probe_math.argtypes = [i, i, sz, vp, vp, vp]
+        L.jaero_probe_osc.argtypes = [i, i, i, vp, vp, d, vp]
         L.jaero_burst_trident_geometry.argtypes = [vp, vp]
         L.jaero_burst_probe_trident.argtypes = [vp, i, vp, vp, vp, vp, vp, vp]
         L.jaero_rt_create.argtypes = [ctypes.c_double, i, i, ctypes.POINTER(vp)]
@@ -225,6 +227,29 @@ def probe_fastfir(taps, x, nfft, writes, device=0):
     y = np.zeros_like(x)
     _check(lib().jaero_probe_fastfir(int(device), int(nfft), _p(h), len(h), x.shape[0], _p(x), x.shape[1], _p(w), len(w), _p(y)))
     return y
+
+
+def probe_math(op, a, b=None, device=0):
+    """test support: out[i] = op(a[i], b[i]) for a device arithmetic primitive as the product compiles it (include/jaero_b200.h,
+    jaero_probe_math; op a JAERO_MATH_* code, 0 .. 8). Integer results come back as doubles."""
+    a = np.ascontiguousarray(a, dtype=np.float64).ravel()
+    if b is not None:
+        b = np.ascontiguousarray(b, dtype=np.float64).ravel()
+        assert b.shape == a.shape
+    out = np.empty_like(a)
+    _check(lib().jaero_probe_math(int(device), int(op), len(a), _p(a), None if b is None else _p(b), _p(out)))
+    return out
+
+
+def probe_osc(op, arg, samplerate, device=0):
+    """test support: one WaveTable oscillator per row of op / arg [n_lanes, n_ops] (JAERO_OSC_* codes) through the device Osc
+    helpers (jaero_probe_osc) -> log [n_lanes, n_ops, 7]: ptr, last, step, freq, table index, passed-point flag, fraction"""
+    op = np.ascontiguousarray(op, dtype=np.int32)
+    arg = np.ascontiguousarray(arg, dtype=np.float64)
+    assert op.ndim == 2 and op.shape == arg.shape
+    log = np.empty(op.shape + (7,), dtype=np.float64)
+    _check(lib().jaero_probe_osc(int(device), op.shape[0], op.shape[1], _p(op), _p(arg), float(samplerate), _p(log)))
+    return log
 
 
 class DemodBatch:

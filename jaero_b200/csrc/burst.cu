@@ -499,9 +499,7 @@ burst_back_kernel(const __grid_constant__ BurstParams p, int n)
                     double fc = ((maxtopposhigh + maxtoppos) / 2) * hzperbin;
                     if (fc < (0.75 * p.fb)) fc = 0.75 * p.fb;
                     if (fc > (p.Fs / 2.0 - 0.75 * p.fb)) fc = p.Fs / 2.0 - 0.75 * p.fb;
-                    mc.freq = fc; if (mc.freq < 0) mc.freq = 0;
-                    mc.step = (mc.freq) * ((double)WTSIZE) / ((double)((float)((int)p.Fs)));   // SetFreq(freq,Fs)
-                    while (((int)mc.ptr) >= WTSIZE) mc.ptr -= WTSIZE;
+                    osc_set_freq_wrap(mc, fc, (int)p.Fs);
                     if (p.afc) osc_set_freq(m2, mc.freq, p.Fs);
                     if ((m2.freq - mc.freq) > (p.lockingbw / 2.0)) osc_set_freq(m2, mc.freq + (p.lockingbw / 2.0), p.Fs);
                     if ((m2.freq - mc.freq) < (-p.lockingbw / 2.0)) osc_set_freq(m2, mc.freq - (p.lockingbw / 2.0), p.Fs);

@@ -893,13 +893,13 @@ int jaero_batch_probe_cfe(jaero_batch *b, const double *ring, int oldest, const 
 
 } // extern "C"
 
-// ---- test support: the streaming FFT convolution on caller data (not part of the drop-in surface)
+// ---- test support: kernels on caller data (not part of the drop-in surface)
 namespace {
-struct FirProbe {
+struct Probe {
     int device; cudaStream_t stream;
     std::vector<void *> allocs;
 };
-void fir_probe_destroy(FirProbe *o)
+void probe_destroy(Probe *o)
 {
     cudaSetDevice(o->device);
     if (o->stream) cudaStreamSynchronize(o->stream);
@@ -927,9 +927,9 @@ int jaero_probe_fastfir(int device, int nfft, const double *taps, int K, int n_c
         set_error("jaero_probe_fastfir: the write sizes add up to " + std::to_string(total) + ", not n = " + std::to_string(n));
         return JAERO_E_ARG;
     }
-    CreateGuard<FirProbe> guard(fir_probe_destroy);          // frees the buffers and the stream on every return
+    CreateGuard<Probe> guard(probe_destroy);                 // frees the buffers and the stream on every return
     { int r = guard.begin("jaero_probe_fastfir", device); if (r) return r; }
-    FirProbe *o = guard.obj;
+    Probe *o = guard.obj;
     std::vector<std::complex<double>> h(K);
     for (int k = 0; k < K; k++) h[k] = std::complex<double>(taps[2 * k], taps[2 * k + 1]);
     FastFir f;
@@ -947,6 +947,47 @@ int jaero_probe_fastfir(int device, int nfft, const double *taps, int K, int n_c
         pos += writes[w];
     }
     JB_CUDA(cudaMemcpyAsync(y, dy, C * n * sizeof(double2), cudaMemcpyDeviceToHost, o->stream));
+    JB_CUDA(cudaStreamSynchronize(o->stream));
+    return JAERO_OK;
+}
+
+int jaero_probe_math(int device, int op, size_t n, const double *a, const double *b, double *out)
+{
+    const bool two = op == JAERO_MATH_DIV_EXACT || op == JAERO_MATH_DIV_FAST || op == JAERO_MATH_ATAN2_FAST || op == JAERO_MATH_HYPOT_FAST ||
+                     op == JAERO_MATH_DIV_FAST_CFE;
+    if (op < JAERO_MATH_DIV_EXACT || op > JAERO_MATH_DIV_FAST_CFE) { set_error("jaero_probe_math: unknown op " + std::to_string(op)); return JAERO_E_ARG; }
+    if (!a || !out || (two && !b) || n == 0) { set_error("jaero_probe_math: null argument or n == 0"); return JAERO_E_ARG; }
+    CreateGuard<Probe> guard(probe_destroy);
+    { int r = guard.begin("jaero_probe_math", device); if (r) return r; }
+    Probe *o = guard.obj;
+    double *da = 0, *db = 0, *dout = 0;
+    if (owned_alloc(o, &da, n) || owned_alloc(o, &dout, n) || (two && owned_alloc(o, &db, n))) return JAERO_E_CUDA;
+    JB_CUDA(cudaMemcpyAsync(da, a, n * sizeof(double), cudaMemcpyHostToDevice, o->stream));
+    if (two) JB_CUDA(cudaMemcpyAsync(db, b, n * sizeof(double), cudaMemcpyHostToDevice, o->stream));
+    const bool cfe = op == JAERO_MATH_LOG10_GE1 || op == JAERO_MATH_DIV_FAST_CFE;
+    if ((cfe ? probe_math_cfe_launch : probe_math_launch)(op, n, da, db, dout, o->stream)) return JAERO_E_CUDA;
+    JB_CUDA(cudaMemcpyAsync(out, dout, n * sizeof(double), cudaMemcpyDeviceToHost, o->stream));
+    JB_CUDA(cudaStreamSynchronize(o->stream));
+    return JAERO_OK;
+}
+
+int jaero_probe_osc(int device, int n_lanes, int n_ops, const int32_t *op, const double *arg, double samplerate, double *log)
+{
+    if (!op || !arg || !log || n_lanes <= 0 || n_ops <= 0) { set_error("jaero_probe_osc: null argument or bad n_lanes / n_ops"); return JAERO_E_ARG; }
+    if (!(samplerate > 0)) { set_error("jaero_probe_osc: samplerate must be positive"); return JAERO_E_ARG; }
+    const size_t n = (size_t)n_lanes * n_ops;
+    for (size_t e = 0; e < n; e++)
+        if (op[e] < JAERO_OSC_SET_FREQ || op[e] > JAERO_OSC_SET_FREQ_SR) {
+            set_error("jaero_probe_osc: unknown op " + std::to_string(op[e]) + " at " + std::to_string(e)); return JAERO_E_ARG; }
+    CreateGuard<Probe> guard(probe_destroy);
+    { int r = guard.begin("jaero_probe_osc", device); if (r) return r; }
+    Probe *o = guard.obj;
+    int32_t *dop = 0; double *darg = 0, *dlog = 0;
+    if (owned_alloc(o, &dop, n) || owned_alloc(o, &darg, n) || owned_alloc(o, &dlog, 7 * n)) return JAERO_E_CUDA;
+    JB_CUDA(cudaMemcpyAsync(dop, op, n * sizeof(int32_t), cudaMemcpyHostToDevice, o->stream));
+    JB_CUDA(cudaMemcpyAsync(darg, arg, n * sizeof(double), cudaMemcpyHostToDevice, o->stream));
+    if (probe_osc_launch(n_lanes, n_ops, dop, darg, samplerate, dlog, o->stream)) return JAERO_E_CUDA;
+    JB_CUDA(cudaMemcpyAsync(log, dlog, 7 * n * sizeof(double), cudaMemcpyDeviceToHost, o->stream));
     JB_CUDA(cudaStreamSynchronize(o->stream));
     return JAERO_OK;
 }

@@ -231,8 +231,9 @@ __device__ __forceinline__ int cc_ph(int e) { return e + (e >> 3); }          //
 
 // log10 for finite x >= 1 (the argument is max(|X|^2, 1)): fdlibm's log kernel — x = 2^k m, m in [sqrt(1/2), sqrt(2)),
 // s = (m-1)/(m+1), degree-14 polynomial in s — with the quotient by div_fast and the final scaling split as in fdlibm's
-// e_log10.c. Within 2 ulp of glibc's log10 on 5 M arguments in [1, 1e40] (host twin: tools/micro/log10_test.c; the library call it
-// replaces is itself only specified to 1 ulp), about half the instructions; the smoothed spectrum feeds an arg-max over
+// e_log10.c. Within 2 ulp of glibc's log10 over [1, DBL_MAX] as this unit compiles it, with contraction, exactly k at 10^k
+// (tests/test_gpu_math.py; host twin without contraction: tools/micro/log10_test.c; the library call it replaces is itself
+// only specified to 1 ulp), about half the instructions; the smoothed spectrum feeds an arg-max over
 // sums of six bins, where differences of that size cannot matter unless the library's own rounding would.
 __device__ __forceinline__ double log10_ge1(double x)
 {
@@ -554,6 +555,27 @@ int cfe_run(const CfePlan &pl, const DemodParams &p, int oldest, cudaStream_t s,
     }
     cfe_search_kernel<<<(C + 3) / 4, 128, 0, s>>>(pl, p);
     *launches += 1;
+    JB_CUDA(cudaGetLastError());
+    return 0;
+}
+
+} // namespace jb
+
+// ---- test support (jaero_probe_math): log10_ge1 and div_fast as this unit compiles them (without -fmad=false)
+#include "../../include/jaero_b200.h"
+
+namespace jb {
+
+__global__ void probe_math_cfe_kernel(int op, size_t n, const double *__restrict__ a, const double *__restrict__ b, double *__restrict__ out)
+{
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+        out[i] = op == JAERO_MATH_LOG10_GE1 ? log10_ge1(a[i]) : div_fast(a[i], b[i]);
+}
+
+int probe_math_cfe_launch(int op, size_t n, const double *a, const double *b, double *out, cudaStream_t s)
+{
+    const size_t blocks = (n + 255) / 256;
+    probe_math_cfe_kernel<<<(unsigned)(blocks < 4096 ? blocks : 4096), 256, 0, s>>>(op, n, a, b, out);
     JB_CUDA(cudaGetLastError());
     return 0;
 }

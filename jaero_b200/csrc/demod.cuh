@@ -110,6 +110,12 @@ int oqpsk_segment_launch(const DemodParams &p, const SegmentArgs &a, const int16
 int oqpsk_pipe_launch(const DemodParams &p, const SegmentArgs &a, const int16_t *d_pcm, size_t stride, cudaStream_t s);
 int msk_pipe_launch(const DemodParams &p, const SegmentArgs &a, const int16_t *d_pcm, size_t stride, cudaStream_t s);
 
+// test support (jaero_probe_math / jaero_probe_osc): the device arithmetic primitives of demod_device.cuh on caller operands, each
+// compiled in the unit whose flags the product builds it with. op is a JAERO_MATH_* / JAERO_OSC_* code of include/jaero_b200.h.
+int probe_math_launch(int op, size_t n, const double *a, const double *b, double *out, cudaStream_t s);       // demod_kernels.cu
+int probe_math_cfe_launch(int op, size_t n, const double *a, const double *b, double *out, cudaStream_t s);   // cfe.cu
+int probe_osc_launch(int n_lanes, int n_ops, const int32_t *op, const double *arg, double samplerate, double *log, cudaStream_t s);
+
 // K2: coarse frequency estimate for every channel of a batch (coarsefreqestimate.cpp:90-137)
 struct CfePlan {
     int nfft, n1, n2, startbin, stopbin, expectedpeakbin, lo, hi, is8400;

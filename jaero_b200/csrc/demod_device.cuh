@@ -4,6 +4,7 @@
 // reference rounds it; the only arithmetic that can differ in the last ulp is libm
 // (hypot / atan2 / tanh / cos / sin / log10).
 #pragma once
+#include <climits>
 #include "demod.cuh"
 #include "common.cuh"
 #include "fft_device.cuh"                  // c_mul
@@ -12,8 +13,9 @@ namespace jb {
 
 // x / d, correctly rounded, for a divisor whose reciprocal rcp = RN(1/d) is loop-invariant (Markstein's sequence:
 // q = RN(x*rcp), r = x - q*d exactly by FMA, result RN(q + r*rcp)). Same value as the IEEE division the reference
-// performs (checked against 3e8 random operands for every divisor used here), in 3 dependent instructions instead of
-// the ~25-deep DDIV expansion. The only deviation: a zero result is always +0.
+// performs wherever that quotient is a normal double (tests/test_gpu_math.py: near-midpoint numerators for every divisor the
+// library derives and every integer divisor up to 2^17), in 3 dependent instructions instead of the ~25-deep DDIV expansion.
+// Deviations: -0 / d gives +0, and a subnormal quotient, whose remainder is not exact, may be 1 ulp off.
 __device__ __forceinline__ double div_exact(double x, double d, double rcp)
 {
     const double q = x * rcp;
@@ -33,7 +35,9 @@ __device__ __forceinline__ double fmod360(double p)
 // these keep the same error class (<= 2 ulp, i.e. the same last-bit differences from glibc that the library calls have) with
 // about half the chain length. Zero / non-finite arguments go to the library call, so the special cases are the library's.
 
-// a / b for finite a and normal positive b: reciprocal seed + two Newton steps + one correction step (<= 1 ulp, usually exact)
+// a / b for finite a and normal positive b: reciprocal seed + two Newton steps + one correction step. The IEEE quotient on the
+// operands of its call sites (tests/test_gpu_math.py: the AGC gain, the log10_ge1 and atan2_fast reductions); where the
+// remainder a - q b underflows (|a| below about 2^-968) or the quotient is subnormal it may be 1 ulp off.
 __device__ __forceinline__ double div_fast(double a, double b)
 {
     double r;
@@ -44,7 +48,8 @@ __device__ __forceinline__ double div_fast(double a, double b)
     return __fma_rn(__fma_rn(-q, b, a), r, q);
 }
 // atan2(y, x) (std::arg of the timing-error phasor, oqpskdemodulator.cpp:480). fdlibm's scheme with ONE division: the argument
-// reduction (t-c)/(1+tc) of t = min/max is formed directly from min and max.
+// reduction (t-c)/(1+tc) of t = min/max is formed directly from min and max. <= 1 ulp from glibc, <= 1.5 ulp from atan2l
+// (tests/test_gpu_math.py).
 __device__ __forceinline__ double atan2_fast(double y, double x)
 {
     const double ax = fabs(x), ay = fabs(y);
@@ -75,16 +80,24 @@ struct Osc {                       // WaveTable (DSP.h:40-81)
     double ptr, step, freq, last;
 };
 
+// (int)d as the reference's x86-64 build converts it (cvttsd2si): truncation where -2^31 - 1 < d < 2^31, INT_MIN for every
+// other value and for NaN. A bare (int)d on the device saturates instead, and gives 0 for NaN.
+__device__ __forceinline__ int x86_int(double d)
+{
+    return (d > -2147483649.0 && d < 2147483648.0) ? (int)d : INT_MIN;
+}
 __device__ __forceinline__ int osc_index(double ptr)                 // DSP.cpp:81-83
 {
     // (int)ptr for 0 <= ptr < 2^31 without the FP64 -> int conversion (50 cycles on this part): adding 2^52 leaves the
     // round-to-nearest integer in the low word; one step down where that rounded up gives the truncation, exactly.
+    // Elsewhere x86's (int)ptr is 0 on (-1, 0), 2^31 - 1 on [2^31 - 1, 2^31) (both give entry 0) and negative or INT_MIN for
+    // every other value and NaN (entry WTSIZE - 1): two compares give the same entry without converting.
     int t;
     if (ptr >= 0.0 && ptr < 2147483647.0) {
         const double m = ptr + 4503599627370496.0;
         t = __double2loint(m);
         if ((m - 4503599627370496.0) > ptr) t -= 1;
-    } else t = (int)ptr;
+    } else t = (ptr > -1.0 && ptr < 2147483648.0) ? 0 : -1;
     if (t >= WTSIZE) t = 0;
     if (t < 0) t = WTSIZE - 1;
     return t;
@@ -95,22 +108,47 @@ __device__ __forceinline__ void osc_set_freq(Osc &o, double f, double samplerate
     if (o.freq < 0) o.freq = 0;
     o.step = div_exact((o.freq) * ((double)WTSIZE), samplerate, 1.0 / samplerate);
 }
+// SetFreq(freq, samplerate) (DSP.cpp:143-149): the quotient by (float)samplerate, then the pointer wrap. The demodulator loops
+// call SetFreq(freq) (osc_set_freq); this form only where the reference re-centres mixer_center (CenterFreqChangedSlot).
+__device__ __forceinline__ void osc_set_freq_wrap(Osc &o, double f, int samplerate)
+{
+    o.freq = f;
+    if (o.freq < 0) o.freq = 0;
+    o.step = (o.freq) * ((double)WTSIZE) / ((double)((float)samplerate));
+    while (x86_int(o.ptr) >= WTSIZE) o.ptr -= WTSIZE;
+}
+// `while(((int)WTptr)>=WTSIZE) WTptr-=WTSIZE;` for a pointer p0 >= WTSIZE that one subtraction left at p >= WTSIZE: with x86's
+// (int), (int)x >= WTSIZE  <=>  WTSIZE <= x < 2^31, so the reference wraps on from p below 2^31 and leaves a larger p0 (+inf
+// included, where a loop on x >= WTSIZE alone would never end) as it was
+__device__ __forceinline__ double osc_wrap_on(double p0, double p)
+{
+    if (!(p0 < 2147483648.0)) return p0;
+    while (p >= (double)WTSIZE) p -= WTSIZE;
+    return p;
+}
 __device__ __forceinline__ void osc_next_frame(Osc &o)               // DSP.cpp:70-77
 {
     if (o.step < 0) o.step = 0;
     o.last = o.ptr;
     o.ptr += o.step;
-    // `while(((int)WTptr)>=WTSIZE)`: for the non-negative finite pointer, (int)x >= N  <=>  x >= (double)N. The step is below N
-    // (frequencies below Fs), so the loop body runs at most once: written as a branch around the (then idle) loop, which costs
-    // a compare instead of a divergent loop on every sample
-    if (o.ptr >= (double)WTSIZE) { o.ptr -= WTSIZE; while (o.ptr >= (double)WTSIZE) o.ptr -= WTSIZE; }
+    // `while(((int)WTptr)>=WTSIZE)`: the step is below WTSIZE (frequencies below Fs), so one subtraction is the whole wrap:
+    // written as a branch around the (then idle) loop, which costs a compare instead of a divergent loop on every sample
+    if (o.ptr >= (double)WTSIZE) {
+        const double p0 = o.ptr;
+        o.ptr -= WTSIZE;
+        if (o.ptr >= (double)WTSIZE) o.ptr = osc_wrap_on(p0, o.ptr);
+    }
 }
 // table index the oscillator will have after its next WTnextFrame(), without committing the advance
 __device__ __forceinline__ int osc_next_index(const Osc &o)
 {
     double s = o.step; if (s < 0) s = 0;
     double q = o.ptr + s;
-    if (q >= (double)WTSIZE) { q -= WTSIZE; while (q >= (double)WTSIZE) q -= WTSIZE; }
+    if (q >= (double)WTSIZE) {                                        // as osc_next_frame
+        const double q0 = q;
+        q -= WTSIZE;
+        if (q >= (double)WTSIZE) q = osc_wrap_on(q0, q);
+    }
     return osc_index(q);
 }
 __device__ __forceinline__ void osc_set_phase_deg(Osc &o, double p)  // DSP.cpp:175-180
@@ -163,10 +201,17 @@ __device__ __forceinline__ double biquad_update(Biquad &q, double sig, double a1
     return y;
 }
 
-// qRound (Qt5 qglobal.h) as used at oqpskdemodulator.cpp:569 / mskdemodulator.cpp:453
+// qRound (Qt5 qglobal.h) as used at oqpskdemodulator.cpp:569 / mskdemodulator.cpp:453, with the reference's x86 conversions
+// (so d >= 2^31 gives INT_MIN, soft bit 0, as there) and its wrapping int addition
 __device__ __forceinline__ int q_round(double d)
 {
-    return d >= 0.0 ? int(d + 0.5) : int(d - double(int(d - 1)) + 0.5) + int(d - 1);
+    if (d >= 0.0) {
+        const double s = d + 0.5;                                    // >= 0.5: only the upper bound of x86_int can fail
+        return s < 2147483648.0 ? (int)s : INT_MIN;
+    }
+    const double e = d - 1;                                          // < -1: only the lower bound can fail (or NaN)
+    const int k = e > -2147483649.0 ? (int)e : INT_MIN;
+    return (int)((unsigned)x86_int(d - double(k) + 0.5) + (unsigned)k);
 }
 
 __device__ __forceinline__ void push_soft(const DemodParams &p, int ch, int &count, int &pending, int &overflow, int ibit)

@@ -335,7 +335,7 @@ oqpsk_pipe_kernel(const __grid_constant__ DemodParams p, const SegmentArgs a, co
                 {   // AGC::Update (DSP.cpp:370-379)
                     ma_push(agc_sum, t_agc[rslot], dabval);
                     ring_dirty = true;
-                    agc_val = div_fast(1.414213562, fmax(div_exact(agc_sum, (double)agc_len, r_agc), 0.000001));   // == the IEEE quotient (tools/micro/div_test.cu)
+                    agc_val = div_fast(1.414213562, fmax(div_exact(agc_sum, (double)agc_len, r_agc), 0.000001));   // == the IEEE quotient (tests/test_gpu_math.py)
                     agc_val = fmax(agc_val, 0.000001);
                 }
                 double2 sig2 = make_double2(sre * agc_val, sim * agc_val);        // :466

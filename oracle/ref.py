@@ -44,6 +44,8 @@ def lib():
         L.jref_trig_tables.argtypes = [vp, vp]
         L.jref_fir.argtypes = [vp, i, vp, vp, l]
         L.jref_qround.argtypes = [d]
+        if hasattr(L, "jref_wavetable_script"):         # absent from a reference build made before it existed
+            L.jref_wavetable_script.argtypes = [i, i, vp, vp, d, vp]
         L.jref_fft.argtypes = [i, i, vp, vp]
         L.jref_fftr_forward.argtypes = [i, vp, vp]
         L.jref_fftr_inverse.argtypes = [i, vp, vp]
@@ -85,6 +87,22 @@ def fastfir_lib():
 
 def _p(a):
     return a.ctypes.data_as(ctypes.c_void_p)
+
+
+def wavetable_script_available():
+    return available() and hasattr(lib(), "jref_wavetable_script")
+
+
+def wavetable_script(op, arg, samplerate):
+    """The reference's own WaveTable (DSP.cpp) running one script per row of op / arg [n_lanes, n_ops] (JAERO_OSC_* codes) ->
+    log [n_lanes, n_ops, 9]: WTptr, last_WTptr, WTstep, freq, table index, IfHavePassedPoint, FractionOfSampleItPassesBy,
+    WTCISValue() re, im (ref_driver.cpp jref_wavetable_script)"""
+    op = np.ascontiguousarray(op, dtype=np.int32)
+    arg = np.ascontiguousarray(arg, dtype=np.float64)
+    assert op.ndim == 2 and op.shape == arg.shape
+    log = np.zeros(op.shape + (9,), dtype=np.float64)
+    lib().jref_wavetable_script(op.shape[0], op.shape[1], _p(op), _p(arg), float(samplerate), _p(log))
+    return log
 
 
 class RefDemod:

@@ -266,6 +266,40 @@ void jref_fir(const double *taps, int ntaps, const double *x, double *y, long n)
     for (long i = 0; i < n; i++) y[i] = f.FIRUpdateAndProcess(x[i]);
 }
 int jref_qround(double d) { return qRound(d); }
+// n_lanes WaveTables, each running its own script: lane l's k-th operation is op[l*n_ops + k] with argument arg[l*n_ops + k]
+// (the JAERO_OSC_* codes of include/jaero_b200.h: 0 SetFreq(a), 1 WTnextFrame(), 2 the index of WTCISValue() one frame ahead on a
+// copy, 3 IncresePhaseDeg(a), 4 SetPhaseDeg(a), 5 AdvanceFractionOfWave(a), 6 IfHavePassedPoint(a), 7 SetFreq(a, samplerate)).
+// Every lane starts with WTptr = last_WTptr = WTstep = freq = 0 at `samplerate`. After each operation
+// log[(l*n_ops + k)*9 + f] holds f = 0 WTptr, 1 last_WTptr, 2 WTstep, 3 freq, 4 the index WTCISValue() read (tint),
+// 5 what IfHavePassedPoint returned (0 for the other ops), 6 FractionOfSampleItPassesBy, 7-8 WTCISValue() (re, im).
+void jref_wavetable_script(int n_lanes, int n_ops, const int32_t *op, const double *arg, double samplerate, double *log)
+{
+    for (int l = 0; l < n_lanes; l++) {
+        WaveTable w;
+        w.samplerate = samplerate; w.freq = 0; w.WTstep = 0; w.WTptr = 0; w.last_WTptr = 0; w.FractionOfSampleItPassesBy = 0;
+        for (int k = 0; k < n_ops; k++) {
+            const size_t e = (size_t)l * n_ops + k;
+            const double a = arg[e];
+            bool flag = false;
+            cpx_type v;
+            int tint;
+            switch (op[e]) {
+            case 0: w.SetFreq(a); break;
+            case 1: w.WTnextFrame(); break;
+            case 3: w.IncresePhaseDeg(a); break;
+            case 4: w.SetPhaseDeg(a); break;
+            case 5: w.AdvanceFractionOfWave(a); break;
+            case 6: flag = w.IfHavePassedPoint(a); break;
+            case 7: w.SetFreq(a, (int)samplerate); break;
+            }
+            if (op[e] == 2) { WaveTable c = w; c.WTnextFrame(); v = c.WTCISValue(); tint = c.tint; }
+            else { v = w.WTCISValue(); tint = w.tint; }
+            double *g = log + e * 9;
+            g[0] = w.WTptr; g[1] = w.last_WTptr; g[2] = w.WTstep; g[3] = w.freq; g[4] = tint; g[5] = flag ? 1.0 : 0.0;
+            g[6] = w.FractionOfSampleItPassesBy; g[7] = v.real(); g[8] = v.imag();
+        }
+    }
+}
 
 // ---------------- FFT wrappers (fftwrapper.cpp, fftrwrapper.cpp) ----------------
 void jref_fft(int nfft, int inverse, const double *in_ri, double *out_ri)
