@@ -438,6 +438,16 @@ class ViterbiBatch:
             pass
 
 
+def _pack_soft(n, soft_list):
+    """per-channel soft-bit arrays -> (buf[n, cap] int16 zero-padded to the longest, cap, counts[n]) for *_process_softbits"""
+    cap = max(1, max(len(s) for s in soft_list))
+    buf = np.zeros((n, cap), dtype=np.int16)
+    counts = np.zeros(n, dtype=np.int32)
+    for c, s in enumerate(soft_list):
+        buf[c, :len(s)] = s; counts[c] = len(s)
+    return buf, cap, counts
+
+
 class PChannelBatch:
     """Batched AeroL P-channel frame layer (600/1200/10500 bps, continuous): soft bits -> CRC-checked SUs + DCD."""
 
@@ -451,11 +461,7 @@ class PChannelBatch:
         _check(lib().jaero_pchannel_process_batch(self.h, batch.h))
 
     def process_softbits(self, soft_list):
-        cap = max(1, max(len(s) for s in soft_list))
-        buf = np.zeros((self.n, cap), dtype=np.int16)
-        counts = np.zeros(self.n, dtype=np.int32)
-        for c, s in enumerate(soft_list):
-            buf[c, :len(s)] = s; counts[c] = len(s)
+        buf, cap, counts = _pack_soft(self.n, soft_list)
         _check(lib().jaero_pchannel_process_softbits(self.h, _p(buf), cap, _p(counts)))
 
     def tick(self, batch=None):
@@ -628,11 +634,7 @@ class RTChannelBatch:
 
     def process(self, soft_list):
         """soft_list: one int16 array per channel."""
-        cap = max(1, max(len(s) for s in soft_list))
-        buf = np.zeros((self.n, cap), dtype=np.int16)
-        counts = np.zeros(self.n, dtype=np.int32)
-        for c, s in enumerate(soft_list):
-            buf[c, :len(s)] = s; counts[c] = len(s)
+        buf, cap, counts = _pack_soft(self.n, soft_list)
         _check(lib().jaero_rt_process_softbits(self.h, _p(buf), cap, _p(counts)))
 
     def process_burst(self, burst_batch):
@@ -690,11 +692,7 @@ class CChannelBatch:
         _check(lib().jaero_cchannel_create(n_channels, device, ctypes.byref(self.h)))
 
     def process(self, soft_list):
-        cap = max(1, max(len(s) for s in soft_list))
-        buf = np.zeros((self.n, cap), dtype=np.int16)
-        counts = np.zeros(self.n, dtype=np.int32)
-        for c, s in enumerate(soft_list):
-            buf[c, :len(s)] = s; counts[c] = len(s)
+        buf, cap, counts = _pack_soft(self.n, soft_list)
         _check(lib().jaero_cchannel_process_softbits(self.h, _p(buf), cap, _p(counts)))
 
     def process_batch(self, batch):

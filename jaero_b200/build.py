@@ -15,9 +15,7 @@ UNITS = [
     ("capi.cu", []),
     ("viterbi.cu", []),
     ("cfe.cu", []),
-    ("pchannel.cu", []),
-    ("rtchannel.cu", []),
-    ("cchannel.cu", []),
+    ("frame_layers.cu", []),
     ("reassembly.cu", []),
     ("ddc.cu", []),
     ("scan.cu", []),

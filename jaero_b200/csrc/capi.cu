@@ -8,10 +8,8 @@
 #include "demod.cuh"
 #include "demod_stages.cuh"                   // msk_half_symbol_delay
 #include "prefilter.cuh"
-#include "pchannel.cuh"
 #include "burst.cuh"
-#include "rtchannel.cuh"
-#include "cchannel.cuh"
+#include "frame_layers.cuh"
 #include "ddc.cuh"
 #include "scan.cuh"
 #include <cstring>
@@ -245,15 +243,6 @@ void host_fft(std::vector<std::complex<double>> &H, const std::vector<std::compl
     for (int len = 2; len <= NF; len <<= 1)
         for (int i = 0; i < NF; i += len)
             for (int k = 0; k < len / 2; k++) { auto w = tw[k * (NF / len)]; auto u = H[i + k], v = H[i + k + len / 2] * w; H[i + k] = u + v; H[i + k + len / 2] = u - v; }
-}
-
-// AeroLScrambler::pre_state (aerol.h:397-437): the first 5000 bits of the scrambler sequence
-std::vector<uint8_t> aerol_scrambler_sequence()
-{
-    int st[15] = {1, 1, 0, 1, 0, 0, 1, 0, 1, 0, 1, 1, 0, 0, 1};
-    std::vector<uint8_t> seq(5000);
-    for (int a = 0; a < 5000; a++) { const int v = st[0] ^ st[14]; seq[a] = (uint8_t)v; for (int i = 14; i > 0; i--) st[i] = st[i - 1]; st[0] = v; }
-    return seq;
 }
 
 template <class T> int dev_alloc_zero(T **p, size_t count, cudaStream_t s)
@@ -1268,11 +1257,6 @@ struct jaero_pchannel : FrameLayer<PChanParams, PChanState> {};
 struct jaero_cchannel : FrameLayer<CChanParams, CChanState> {};
 
 namespace {
-__global__ void pchan_su_reset_kernel(PChanParams pp)
-{
-    const int ch = blockIdx.x * blockDim.x + threadIdx.x;
-    if (ch < pp.n_channels) { pp.state[ch].su_count = 0; pp.state[ch].queue_overflow = 0; }
-}
 // a call is about to launch on a batch's stream `bs`: order it behind whatever this layer queued on its own stream
 template <class L> int pc_enter(L *p, cudaStream_t bs)
 {
@@ -1338,14 +1322,15 @@ template <class L> int layer_process_softbits(L *l, const int16_t *soft, size_t 
     JB_CUDA(cudaStreamSynchronize(l->stream));
     return JAERO_OK;
 }
-// tick and lost_signal: one launch that may write the demodulator's DCD, on the batch's stream when a batch is given (b may be
-// NULL: frame layer only). tick passes channel -1.
-template <class L, class F> int layer_dcd_launch(L *l, jaero_batch *b, int channel, const char *fn, F launch)
+// tick and lost_signal: launch(state, n_channels, args..., demod_dcd, stream), which may write the demodulator's DCD, on the
+// batch's stream when a batch is given (b may be NULL: frame layer only). tick passes channel -1.
+template <class L, class F, class... A> int layer_dcd_launch(L *l, jaero_batch *b, int channel, const char *fn, F launch, A... args)
 {
     if (!l || channel >= l->params.n_channels || (b && b->p.n_channels != l->params.n_channels)) { set_error(std::string(fn) + ": bad argument"); return JAERO_E_ARG; }
     JB_CUDA(cudaSetDevice(l->device));
     if (b) { if (pc_enter(l, b->stream)) return JAERO_E_CUDA; } else l->own_dirty = true;
-    if (launch(l->params, b ? b->p.I + (size_t)I_DCD * b->p.cpad : nullptr, b ? b->stream : l->stream)) return JAERO_E_CUDA;
+    int *dcd = b ? b->p.I + (size_t)I_DCD * b->p.cpad : nullptr;
+    if (launch(l->params.state, l->params.n_channels, args..., dcd, b ? b->stream : l->stream)) return JAERO_E_CUDA;
     l->launches++;
     return (b && pc_leave(l, b->stream)) ? JAERO_E_CUDA : JAERO_OK;
 }
@@ -1462,8 +1447,7 @@ int jaero_pchannel_create(int n_channels, double fb, int device, jaero_pchannel 
     rc |= owned_alloc(p, &p->vit_renorm, C);
     rc |= owned_alloc(p, &p->vit_valid, C);
     if (rc) return JAERO_E_CUDA;
-    if (pchan_set_scrambler(aerol_scrambler_sequence().data())) return JAERO_E_CUDA;
-    if (pchan_init(pp, p->stream)) return JAERO_E_CUDA;
+    if (frame_set_scrambler() || per_channel_launch(pchan_init_kernel, n_channels, p->stream, pp)) return JAERO_E_CUDA;
     JB_CUDA(cudaStreamSynchronize(p->stream));
     JB_CUDA(cudaMallocHost(&p->h_state, C * sizeof(PChanState)));
     JB_CUDA(cudaMallocHost(&p->h_out, C * pp.su_cap * 16));
@@ -1479,13 +1463,12 @@ int jaero_pchannel_process_softbits(jaero_pchannel *p, const int16_t *soft, size
 {
     return layer_process_softbits(p, soft, cap, counts, "jaero_pchannel_process_softbits");
 }
-int jaero_pchannel_tick(jaero_pchannel *p, jaero_batch *b) { return layer_dcd_launch(p, b, -1, "jaero_pchannel_tick", pchan_tick); }
+int jaero_pchannel_tick(jaero_pchannel *p, jaero_batch *b) { return layer_dcd_launch(p, b, -1, "jaero_pchannel_tick", frame_tick<PChanState>); }
 // AeroL::SignalStatusSlot(false) -> LostSignal() (aerol.h:920-931): cntr = 1e9, DCD countdown and DCD cleared at once, and
 // DataCarrierDetect(false) reaches the demodulator (b may be NULL: frame layer only). channel -1 = every channel.
 int jaero_pchannel_lost_signal(jaero_pchannel *p, jaero_batch *b, int channel)
 {
-    return layer_dcd_launch(p, b, channel, "jaero_pchannel_lost_signal",
-                            [channel](const PChanParams &pp, int *dcd, cudaStream_t s) { return pchan_lost(pp, channel, dcd, s); });
+    return layer_dcd_launch(p, b, channel, "jaero_pchannel_lost_signal", frame_lost<PChanState>, channel);
 }
 int jaero_pchannel_write_batch(jaero_pchannel *p, jaero_batch *b, const int16_t *pcm, size_t n, size_t stride)
 {
@@ -1505,8 +1488,7 @@ int jaero_pchannel_read_sus(jaero_pchannel *p, uint8_t *out, size_t cap, int32_t
         counts[ch] = p->h_state[ch].su_count;
         if (counts[ch]) memcpy(out + (size_t)ch * cap * 16, p->h_out + (size_t)ch * pp.su_cap * 16, (size_t)counts[ch] * 16);
     }
-    pchan_su_reset_kernel<<<(pp.n_channels + 127) / 128, 128, 0, p->stream>>>(pp);
-    JB_CUDA(cudaGetLastError());
+    if (per_channel_launch(pchan_su_reset_kernel, pp.n_channels, p->stream, pp)) return JAERO_E_CUDA;
     p->own_dirty = true;
     return JAERO_OK;
 }
@@ -1514,8 +1496,7 @@ int jaero_pchannel_discard_sus(jaero_pchannel *p)
 {
     if (!p) { set_error("null handle"); return JAERO_E_ARG; }
     JB_CUDA(cudaSetDevice(p->device));
-    pchan_su_reset_kernel<<<(p->params.n_channels + 127) / 128, 128, 0, p->stream>>>(p->params);
-    JB_CUDA(cudaGetLastError());
+    if (per_channel_launch(pchan_su_reset_kernel, p->params.n_channels, p->stream, p->params)) return JAERO_E_CUDA;
     p->own_dirty = true;
     p->launches++;
     return JAERO_OK;
@@ -1892,8 +1873,7 @@ int jaero_rt_create(double fb, int n_channels, int device, jaero_rt **out)
     rc |= owned_alloc(r, &rp.state, C); rc |= owned_alloc(r, &rp.slots, C * RT_SLOTS); rc |= owned_alloc(r, &rp.blocks, C * RT_SLOTS * RT_BLOCK);
     rc |= owned_alloc(r, &rp.out, C * RT_OUT * RT_OUT_BYTES);
     if (rc) return JAERO_E_CUDA;
-    if (rt_set_scrambler(aerol_scrambler_sequence().data())) return JAERO_E_CUDA;
-    if (rt_init(rp, r->stream)) return JAERO_E_CUDA;
+    if (frame_set_scrambler() || per_channel_launch(rt_init_kernel, n_channels, r->stream, rp)) return JAERO_E_CUDA;
     JB_CUDA(cudaStreamSynchronize(r->stream));
     JB_CUDA(cudaMallocHost(&r->h_state, C * sizeof(RtState)));
     JB_CUDA(cudaMallocHost(&r->h_out, C * RT_OUT * RT_OUT_BYTES));
@@ -1943,7 +1923,7 @@ int jaero_rt_tick(jaero_rt *r)
 {
     if (!r) { set_error("null handle"); return JAERO_E_ARG; }
     JB_CUDA(cudaSetDevice(r->device));
-    if (rt_tick(r->rp, r->stream)) return JAERO_E_CUDA;
+    if (frame_tick(r->rp.state, r->rp.n_channels, nullptr, r->stream)) return JAERO_E_CUDA;
     r->launches++;
     return JAERO_OK;
 }
@@ -1954,7 +1934,7 @@ int jaero_rt_read_packets(jaero_rt *r, uint8_t *out, int cap_packets, int32_t *c
     bool overflow = false;
     if (read_records(r->rp.state, r->h_state, r->rp.out, r->h_out, r->rp.n_channels, RT_OUT, RT_OUT_BYTES, r->stream,
                      out, cap_packets, counts, &overflow)) return JAERO_E_CUDA;
-    if (rt_out_reset(r->rp, r->stream)) return JAERO_E_CUDA;
+    if (frame_out_reset(r->rp.state, r->rp.n_channels, r->stream)) return JAERO_E_CUDA;
     r->launches++;
     if (overflow) { set_error("R/T packet queue overflow: read more often"); return JAERO_E_OVERFLOW; }
     return JAERO_OK;
@@ -1995,8 +1975,7 @@ int jaero_cchannel_create(int n_channels, int device, jaero_cchannel **out)
     rc |= owned_alloc(c, &cp.ready, C); rc |= owned_alloc(c, &cp.dl2, C * cp.dl2_len); rc |= owned_alloc(c, &cp.out, C * CC_OUT * CC_RECORD);
     rc |= owned_alloc(c, &c->vit_overlap, C * 64); rc |= owned_alloc(c, &c->vit_overlap_len, C); rc |= owned_alloc(c, &c->vit_renorm, C); rc |= owned_alloc(c, &c->vit_valid, C);
     if (rc) return JAERO_E_CUDA;
-    if (cchan_set_scrambler(aerol_scrambler_sequence().data())) return JAERO_E_CUDA;
-    if (cchan_init(cp, c->stream)) return JAERO_E_CUDA;
+    if (frame_set_scrambler() || per_channel_launch(cchan_init_kernel, n_channels, c->stream, cp)) return JAERO_E_CUDA;
     JB_CUDA(cudaStreamSynchronize(c->stream));
     JB_CUDA(cudaMallocHost(&c->h_state, C * sizeof(CChanState)));
     JB_CUDA(cudaMallocHost(&c->h_out, C * CC_OUT * CC_RECORD));
@@ -2011,11 +1990,10 @@ int jaero_cchannel_process_softbits(jaero_cchannel *c, const int16_t *soft, size
 {
     return layer_process_softbits(c, soft, cap, counts, "jaero_cchannel_process_softbits");
 }
-int jaero_cchannel_tick(jaero_cchannel *c, jaero_batch *b) { return layer_dcd_launch(c, b, -1, "jaero_cchannel_tick", cchan_tick); }
+int jaero_cchannel_tick(jaero_cchannel *c, jaero_batch *b) { return layer_dcd_launch(c, b, -1, "jaero_cchannel_tick", frame_tick<CChanState>); }
 int jaero_cchannel_lost_signal(jaero_cchannel *c, jaero_batch *b, int channel)     // AeroL::LostSignal, see jaero_pchannel_lost_signal
 {
-    return layer_dcd_launch(c, b, channel, "jaero_cchannel_lost_signal",
-                            [channel](const CChanParams &cp, int *dcd, cudaStream_t s) { return cchan_lost(cp, channel, dcd, s); });
+    return layer_dcd_launch(c, b, channel, "jaero_cchannel_lost_signal", frame_lost<CChanState>, channel);
 }
 int jaero_cchannel_write_batch(jaero_cchannel *c, jaero_batch *b, const int16_t *pcm, size_t n, size_t stride)   // see jaero_pchannel_write_batch
 {
@@ -2028,7 +2006,7 @@ int jaero_cchannel_read_frames(jaero_cchannel *c, uint8_t *out, int cap_frames, 
     bool overflow = false;
     if (read_records(c->params.state, c->h_state, c->params.out, c->h_out, c->params.n_channels, CC_OUT, CC_RECORD, c->stream,
                      out, cap_frames, counts, &overflow)) return JAERO_E_CUDA;
-    if (cchan_out_reset(c->params, c->stream)) return JAERO_E_CUDA;
+    if (frame_out_reset(c->params.state, c->params.n_channels, c->stream)) return JAERO_E_CUDA;
     c->own_dirty = true;
     c->launches++;
     if (overflow) { set_error("C-channel frame queue overflow: read more often"); return JAERO_E_OVERFLOW; }

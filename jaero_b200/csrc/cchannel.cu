@@ -11,20 +11,10 @@
 //   3. cchan_su_kernel      dl2 -> scrambler -> signal units + CRC + DCD -> voice bytes
 // Integer/byte work throughout: bit-exact against the oracle (oracle/restated/fec_oracle.cpp CChannelOracle).
 #include <cstdint>
-#include "common.cuh"
 #include "viterbi.cuh"
-#include "demod.cuh"
-#include "cchannel.cuh"
+#include "frame_stages.cuh"
 
 namespace jb {
-
-__constant__ uint8_t c_cc_scr[5000];
-
-int cchan_set_scrambler(const uint8_t *seq)
-{
-    JB_CUDA(cudaMemcpyToSymbol(c_cc_scr, seq, 5000));
-    return 0;
-}
 
 static const unsigned long long CC_PRE1 = 216866263330005ULL, CC_PRE2 = 3012071630031408ULL;   // aerol.cpp:953-954
 static const unsigned long long CC_MASK = (1ULL << 52) - 1;
@@ -61,28 +51,19 @@ cchan_frame_kernel(CChanParams cp, const int16_t *__restrict__ soft, const int *
         s.carry_slot = 0;
     }
     s.frames_ready = 0;
-    // AeroL::LostSignal (aerol.h:925-931) at the recorded SignalStatus(false) positions
-    int nev = lost_n ? min(lost_n[ch], LOST_CAP) : 0, ev = 0;
-    if (lost_n && lost_n[ch] > LOST_CAP) s.overflow = 1;
-    int next_ev = nev ? lost_pos[ch] : 0x7fffffff;
+    LostCursor lost(lost_n, lost_pos, lost_pitch, ch, s.overflow);
     for (int i = 0; i < n; i++) {
-        while (i >= next_ev) { s.cntr = 1000000000; s.datacdcountdown = 0; s.datacd = 0; ev++; next_ev = ev < nev ? lost_pos[(size_t)ev * lost_pitch + ch] : 0x7fffffff; }
+        lost.take(s, i);
         const int v = bits[i];
         s.bits_seen++;
         int bit = (((unsigned char)v) >= 128) ? 1 : 0;
         int soft_bit = (unsigned short)v;
-        int gotsync = 0;
-        s.realimag++; s.realimag %= 2;
         const bool search = (s.cntr > CC_FRAME_BITS - 112 || s.cntr <= 0);                   // :2212,2236
-        int inv;
-        if (s.realimag) { if (search) gotsync = cc_uw(s.b1_real, s.b2_real, bit, s.inv_real); inv = s.inv_real; }
-        else { if (search) gotsync = cc_uw(s.b1_imag, s.b2_imag, bit, s.inv_imag); inv = s.inv_imag; }
-        if (search) { if (!s.gotsync_last) { s.gotsync_last = gotsync; gotsync = 0; } else s.gotsync_last = 0; }
-        else { gotsync = 0; s.gotsync_last = 0; }
-        if (inv) { bit = 1 - bit; if (soft_bit != 128) soft_bit = 255 - soft_bit; }
+        const int gotsync = oqpsk_arm_search(s.realimag, s.gotsync_last, s.inv_real, s.inv_imag, search, bit, soft_bit,
+            [&](int arm, int b, int &inv) { return arm ? cc_uw(s.b1_real, s.b2_real, b, inv) : cc_uw(s.b1_imag, s.b2_imag, b, inv); });
         if (gotsync) { s.cntr = -1; s.index = -1; }                                           // :2286-2296
         else {
-            if (s.cntr < 1000000000) s.cntr++;
+            if (s.cntr < CNTR_IDLE) s.cntr++;
             if (s.cntr <= CC_FRAME_BITS - 1) {
                 // block[index] -> deinterleave_ba(block,4) -> append -> depuncture: the code-order slot of frame bit c
                 const int c = s.cntr, b = c >> 8, idx = c & 255, r = idx >> 2, j = idx & 3;
@@ -95,24 +76,10 @@ cchan_frame_kernel(CChanParams cp, const int16_t *__restrict__ soft, const int *
             }
         }
     }
-    if (ev < nev) { s.cntr = 1000000000; s.datacdcountdown = 0; s.datacd = 0; }
+    lost.finish(s);
     s.carry_slot = (s.frames_ready > 0 && s.frames_ready < CC_QUEUE) ? s.frames_ready : 0;
     cp.state[ch] = s;
     cp.ready[ch] = s.frames_ready;
-}
-
-__device__ __forceinline__ unsigned cc_crc16(const uint8_t *bytes, int n)      // AeroLcrc16::calcusingbytes (aerol.h:334-362)
-{
-    unsigned crc = 0xFFFF;
-    for (int i = 0; i < n; i++) {
-        unsigned byte = bytes[i];
-        for (int t = 0; t < 8; t++) {
-            const unsigned mb = byte & 1u; byte >>= 1;
-            const unsigned cb = crc & 1u; crc >>= 1;
-            if (cb ^ mb) crc ^= 0x8408u;
-        }
-    }
-    return (~crc) & 0xFFFFu;
 }
 
 __global__ void __launch_bounds__(64)
@@ -128,7 +95,7 @@ cchan_su_kernel(CChanParams cp, int *__restrict__ demod_dcd)
         for (int h = 0; h < CC_KEEP; h++) {
             int b = dec[h];
             dl2[s.dl2_ptr] = (uint8_t)b; s.dl2_ptr++; if (s.dl2_ptr >= cp.dl2_len) s.dl2_ptr = 0; b = dl2[s.dl2_ptr];
-            dec[h] = (uint8_t)(b ^ c_cc_scr[h]);
+            dec[h] = (uint8_t)(b ^ c_scr[h]);
         }
         uint8_t *rec = nullptr;
         if (s.out_count < CC_OUT) rec = cp.out + ((size_t)ch * CC_OUT + s.out_count) * CC_RECORD; else s.overflow = 1;
@@ -141,7 +108,7 @@ cchan_su_kernel(CChanParams cp, int *__restrict__ demod_dcd)
                 if (charptr == 0) { info[ninfo++] = (uint8_t)ch8; ch8 = 0; } else ch8 >>= 1;
             }
             if (ninfo == 12) {
-                const unsigned crc_calc = cc_crc16(info, 10);
+                const unsigned crc_calc = crc16_bytes(info, 10);
                 const unsigned crc_rec = ((unsigned)info[11] << 8) | info[10];
                 const int ok = crc_calc == crc_rec;
                 if (ok) { if (s.datacdcountdown < 12) s.datacdcountdown += 2; }
@@ -168,66 +135,18 @@ cchan_su_kernel(CChanParams cp, int *__restrict__ demod_dcd)
     if (demod_dcd) demod_dcd[ch] = s.datacd;
 }
 
-__global__ void cchan_tick_kernel(CChanParams cp, int *demod_dcd)             // AeroL::updateDCD (aerol.cpp:1109-1122)
-{
-    const int ch = blockIdx.x * blockDim.x + threadIdx.x;
-    if (ch >= cp.n_channels) return;
-    CChanState &s = cp.state[ch];
-    if (s.datacdcountdown > 0) s.datacdcountdown -= 3;
-    else { if (s.datacdcountdown < 0) s.datacdcountdown = 0; }
-    if (s.datacd && !s.datacdcountdown) s.datacd = 0;
-    if (demod_dcd) demod_dcd[ch] = s.datacd;
-}
 __global__ void cchan_init_kernel(CChanParams cp)
 {
     const int ch = blockIdx.x * blockDim.x + threadIdx.x;
     if (ch >= cp.n_channels) return;
     CChanState s;
     memset(&s, 0, sizeof s);
-    s.cntr = 1000000000;                                       // AeroL ctor (aerol.cpp:907,927); index = 0 (:957)
+    s.cntr = CNTR_IDLE;                                        // AeroL ctor (aerol.cpp:907,927); index = 0 (:957)
     cp.state[ch] = s;
     uint8_t *coded = cp.coded + (size_t)ch * CC_QUEUE * CC_CODED_PITCH;
     for (int q = 0; q < CC_QUEUE; q++) for (int k = 0; k < CC_CODED_PITCH; k++) coded[(size_t)q * CC_CODED_PITCH + k] = 128;   // erasure slots
 }
-__global__ void cchan_out_reset_kernel(CChanParams cp)
-{
-    const int ch = blockIdx.x * blockDim.x + threadIdx.x;
-    if (ch >= cp.n_channels) return;
-    cp.state[ch].out_count = 0;
-}
 
-int cchan_init(const CChanParams &cp, cudaStream_t st)
-{
-    cchan_init_kernel<<<(cp.n_channels + 127) / 128, 128, 0, st>>>(cp);
-    JB_CUDA(cudaGetLastError());
-    return 0;
-}
-int cchan_tick(const CChanParams &cp, int *demod_dcd, cudaStream_t st)
-{
-    cchan_tick_kernel<<<(cp.n_channels + 127) / 128, 128, 0, st>>>(cp, demod_dcd);
-    JB_CUDA(cudaGetLastError());
-    return 0;
-}
-int cchan_out_reset(const CChanParams &cp, cudaStream_t st)
-{
-    cchan_out_reset_kernel<<<(cp.n_channels + 127) / 128, 128, 0, st>>>(cp);
-    JB_CUDA(cudaGetLastError());
-    return 0;
-}
-__global__ void cchan_lost_kernel(CChanParams cp, int channel, int *__restrict__ demod_dcd)     // AeroL::LostSignal
-{
-    const int ch = blockIdx.x * blockDim.x + threadIdx.x;
-    if (ch >= cp.n_channels || (channel >= 0 && channel != ch)) return;
-    CChanState &s = cp.state[ch];
-    s.cntr = 1000000000; s.datacdcountdown = 0; s.datacd = 0;
-    if (demod_dcd) demod_dcd[ch] = 0;
-}
-int cchan_lost(const CChanParams &cp, int channel, int *demod_dcd, cudaStream_t st)
-{
-    cchan_lost_kernel<<<(cp.n_channels + 127) / 128, 128, 0, st>>>(cp, channel, demod_dcd);
-    JB_CUDA(cudaGetLastError());
-    return 0;
-}
 int cchan_process(const CChanParams &cp, const int16_t *d_soft, const int *d_soft_count, size_t soft_stride, int *demod_dcd,
                   uint8_t *vit_overlap, int *vit_overlap_len, int *vit_renorm, int *vit_valid, cudaStream_t st, long long *launches,
                   const int *lost_n, const int *lost_pos, size_t lost_pitch)

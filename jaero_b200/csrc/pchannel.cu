@@ -14,31 +14,11 @@
 // updates of datacdcountdown (aerol.cpp:1601-1608) are applied after stage 3, i.e. at the end of the call that
 // completed the frame, not in the middle of the bit loop.
 #include <cstdint>
-#include "common.cuh"
-#include "demod.cuh"
 #include "viterbi.cuh"
-#include "pchannel.cuh"
+#include "frame_stages.cuh"
 
 namespace jb {
 
-__device__ uint8_t g_scr[5000];            // AeroLScrambler::pre_state (global, not constant: it is indexed per lane)
-
-int pchan_set_scrambler(const uint8_t *seq)
-{
-    JB_CUDA(cudaMemcpyToSymbol(g_scr, seq, 5000));
-    return 0;
-}
-
-static const unsigned UWORD = 0xE15AE893u; // aerol.cpp:947
-
-// PreambleDetectorPhaseInvariant::Update with tollerence 0 (aerol.cpp:781-804): the buffer is a 32-bit shift register
-__device__ __forceinline__ int uw_invariant(unsigned &sr, int bit, int &inverted)
-{
-    sr = (sr << 1) | (unsigned)bit;
-    if (sr == ~UWORD) { inverted = 1; return 1; }      // xorsum == 32
-    if (sr == UWORD) { inverted = 0; return 1; }       // xorsum == 0
-    return 0;
-}
 // PreambleDetector::Update (aerol.cpp:744-750): exact match, buffer zeroed on a hit
 __device__ __forceinline__ int uw_exact(unsigned &sr, int bit)
 {
@@ -57,14 +37,15 @@ __device__ __forceinline__ void pchan_frame_bit(const PChanParams &pp, PChanStat
     if (v < 0) return;                                                       // burst marker: never in continuous modes
     int gotsync;
     if (pp.oqpsk) {                                                          // :1156-1233
+        // oqpsk_arm_search written out: through the shared stage (its invert_soft) this kernel's SASS changes
         s.realimag++; s.realimag %= 2;
         const bool search = (s.cntr > pp.number_of_bits - 68 || s.cntr <= 0 || !s.datacd);
         int inv;
         if (s.realimag) {                                                    // explicit arms: the state stays in registers
-            if (search) gotsync = uw_invariant(s.sr_imag, bit, s.inv_imag);
+            if (search) gotsync = uw_phase_invariant<0>(s.sr_imag, bit, s.inv_imag);
             inv = s.inv_imag;
         } else {
-            if (search) gotsync = uw_invariant(s.sr_real, bit, s.inv_real);
+            if (search) gotsync = uw_phase_invariant<0>(s.sr_real, bit, s.inv_real);
             inv = s.inv_real;
         }
         if (search) { if (!s.gotsync_last) { s.gotsync_last = gotsync; gotsync = 0; } else s.gotsync_last = 0; }
@@ -72,7 +53,7 @@ __device__ __forceinline__ void pchan_frame_bit(const PChanParams &pp, PChanStat
         if (inv) { bit = 1 - bit; if (soft_bit != 128) soft_bit = 255 - soft_bit; }
     } else gotsync = uw_exact(s.sr_plain, bit);                              // :1269-1272
 
-    if (s.cntr < 1000000000) s.cntr++;
+    if (s.cntr < CNTR_IDLE) s.cntr++;
     if (s.cntr < 16) {                                                       // :1275-1300
         if (s.cntr == 0) { s.frameinfo = (unsigned short)bit; s.info_len = 0; }
         else s.frameinfo = (unsigned short)((s.frameinfo << 1) | bit);
@@ -82,7 +63,7 @@ __device__ __forceinline__ void pchan_frame_bit(const PChanParams &pp, PChanStat
     }
     if (s.cntr >= 16) {                                                      // :1540-1552
         int idx;                                                             // (cntr-BitsInHeader)%block_len, negative -> 0
-        if (s.cntr >= 1000000000) idx = idle_idx;
+        if (s.cntr >= CNTR_IDLE) idx = idle_idx;
         else { idx = s.cntr - pp.bits_in_header; if (idx < 0) idx = 0; idx %= block_len; }
         // every slot holds a completed block the Viterbi stage has not decoded yet: this bit has nowhere to go. Flag it
         // (read_sus / get_stats report JAERO_E_OVERFLOW) instead of overwriting a queued block.
@@ -153,21 +134,22 @@ pchan_frame_kernel(PChanParams pp, const int16_t *__restrict__ soft, const int *
     const int16_t *bits = soft + (size_t)ch * soft_cap;
     const int block_len = pp.block_len, QD = pp.queue;
     // while the frame counter sits at its idle value 1e9 the block index is the constant (1e9 - BitsInHeader) % block_len
-    const int idle_idx = (1000000000 - pp.bits_in_header) % block_len;
+    const int idle_idx = (CNTR_IDLE - pp.bits_in_header) % block_len;
     s.blocks_ready = 0;
-    // AeroL::LostSignal (aerol.h:925-931) at the soft-bit positions the demodulator recorded its SignalStatus(false) events
+    // AeroL::LostSignal at the soft-bit positions the demodulator recorded its SignalStatus(false) events. LostCursor written
+    // out: through it this kernel's SASS changes.
     int nev = lost_n ? min(lost_n[ch], LOST_CAP) : 0, ev = 0;
     if (lost_n && lost_n[ch] > LOST_CAP) s.queue_overflow = 1;
     int next_ev = nev ? lost_pos[ch] : 0x7fffffff;
     int i = 0;
     while (i < n) {
-        while (i >= next_ev) { s.cntr = 1000000000; s.datacdcountdown = 0; s.datacd = 0; ev++; next_ev = ev < nev ? lost_pos[(size_t)ev * lost_pitch + ch] : 0x7fffffff; }
+        while (i >= next_ev) { lost_signal(s); ev++; next_ev = ev < nev ? lost_pos[(size_t)ev * lost_pitch + ch] : 0x7fffffff; }
         int r = min(32, min(n, next_ev) - i);                                // bits this round may take (>= 1)
         const int v = (lane < r) ? (int)bits[i + lane] : 0;
         const unsigned negm = __ballot_sync(0xffffffffu, v < 0);
         if (negm) r = min(r, __ffs(negm) - 1);
         const int c = s.cntr;
-        const bool idle = (c >= 1000000000);
+        const bool idle = (c >= CNTR_IDLE);
         bool fast = pp.oqpsk && r > 0 && s.blocks_ready < QD;
         bool searching = true;
         int idx0 = idle_idx;
@@ -225,7 +207,7 @@ pchan_frame_kernel(PChanParams pp, const int16_t *__restrict__ soft, const int *
             i++;
         }
     }
-    if (ev < nev) { s.cntr = 1000000000; s.datacdcountdown = 0; s.datacd = 0; }     // events after the last soft bit
+    if (ev < nev) lost_signal(s);                                            // events after the last soft bit
     s.bits_seen += n;
     // carry the partially filled block of slot `blocks_ready` back to slot 0 for the next call
     if (s.blocks_ready > 0 && s.blocks_ready < QD) s.carry_slot = s.blocks_ready; else s.carry_slot = 0;
@@ -285,11 +267,7 @@ pchan_su_kernel(PChanParams pp, int *__restrict__ demod_dcd)
                     for (int i = 0; i < 10; i++) {
                         unsigned byte = su[i];
                         tsum += (int)byte;
-                        for (int t = 0; t < 8; t++) {
-                            const unsigned mb = byte & 1u; byte >>= 1;
-                            const unsigned cb = crc & 1u; crc >>= 1;
-                            if (cb ^ mb) crc ^= 0x8408u;
-                        }
+                        for (int t = 0; t < 8; t++) { crc = crc16_step(crc, byte & 1u); byte >>= 1; }
                     }
                     unsigned crc_calc = (~crc) & 0xFFFFu;
                     const unsigned crc_rec = ((unsigned)su[11] << 8) | su[10];
@@ -334,56 +312,22 @@ pchan_su_kernel(PChanParams pp, int *__restrict__ demod_dcd)
     }
 }
 
-// AeroL::updateDCD (aerol.cpp:1109-1122), the reference's 1 s QTimer
-__global__ void pchan_tick_kernel(PChanParams pp, int *__restrict__ demod_dcd)
-{
-    const int ch = blockIdx.x * blockDim.x + threadIdx.x;
-    if (ch >= pp.n_channels) return;
-    PChanState &s = pp.state[ch];
-    if (s.datacdcountdown > 0) s.datacdcountdown -= 3;
-    else if (s.datacdcountdown < 0) s.datacdcountdown = 0;
-    if (s.datacd && !s.datacdcountdown) s.datacd = 0;
-    if (demod_dcd) demod_dcd[ch] = s.datacd;
-}
-
 __global__ void pchan_init_kernel(PChanParams pp)
 {
     const int ch = blockIdx.x * blockDim.x + threadIdx.x;
     if (ch >= pp.n_channels) return;
     PChanState s;
     memset(&s, 0, sizeof s);
-    s.cntr = 1000000000;                     // aerol.cpp:899
+    s.cntr = CNTR_IDLE;                      // aerol.cpp:899
     s.blockcnt = -1;
     pp.state[ch] = s;
 }
 
-int pchan_init(const PChanParams &pp, cudaStream_t st)
-{
-    pchan_init_kernel<<<(pp.n_channels + 127) / 128, 128, 0, st>>>(pp);
-    JB_CUDA(cudaGetLastError());
-    return 0;
-}
-int pchan_tick(const PChanParams &pp, int *demod_dcd, cudaStream_t st)
-{
-    pchan_tick_kernel<<<(pp.n_channels + 127) / 128, 128, 0, st>>>(pp, demod_dcd);
-    JB_CUDA(cudaGetLastError());
-    return 0;
-}
-
-// AeroL::LostSignal for one channel (>= 0) or all (-1)
-__global__ void pchan_lost_kernel(PChanParams pp, int channel, int *__restrict__ demod_dcd)
+// the signal-unit ring has been read out
+__global__ void pchan_su_reset_kernel(PChanParams pp)
 {
     const int ch = blockIdx.x * blockDim.x + threadIdx.x;
-    if (ch >= pp.n_channels || (channel >= 0 && channel != ch)) return;
-    PChanState &s = pp.state[ch];
-    s.cntr = 1000000000; s.datacdcountdown = 0; s.datacd = 0;
-    if (demod_dcd) demod_dcd[ch] = 0;
-}
-int pchan_lost(const PChanParams &pp, int channel, int *demod_dcd, cudaStream_t st)
-{
-    pchan_lost_kernel<<<(pp.n_channels + 127) / 128, 128, 0, st>>>(pp, channel, demod_dcd);
-    JB_CUDA(cudaGetLastError());
-    return 0;
+    if (ch < pp.n_channels) { pp.state[ch].su_count = 0; pp.state[ch].queue_overflow = 0; }
 }
 
 int pchan_process(const PChanParams &pp, const int16_t *d_soft, const int *d_soft_count, int soft_cap, int *demod_dcd,

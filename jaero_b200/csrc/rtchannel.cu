@@ -14,32 +14,12 @@
 // Known deviation (DESIGN.md): the reference returns from Decode() in the middle of a 32-value vector when the burst
 // time-out fires (aerol.cpp:2018-2027) and so drops the rest of that vector; here the stream is processed without drops.
 #include <cstdint>
-#include "common.cuh"
 #include "viterbi_core.cuh"
-#include "rtchannel.cuh"
+#include "frame_stages.cuh"
 
 namespace jb {
 
-__constant__ uint8_t c_rt_scr[5000];       // AeroLScrambler::pre_state (aerol.h:397-437)
-
-int rt_set_scrambler(const uint8_t *seq)
-{
-    JB_CUDA(cudaMemcpyToSymbol(c_rt_scr, seq, 5000));
-    return 0;
-}
-
-static const unsigned RT_UWORD = 0xE15AE893u;     // aerol.cpp:947
 enum { RT_OK_R = 3, RT_OK_T = 5, RT_BAD = 0, RT_TEST_FAILED = 32, RT_NOTHING = 8 };
-
-// PreambleDetectorPhaseInvariant::Update (aerol.cpp:781-804), tollerence 4, on a 32-bit shift register
-__device__ __forceinline__ int rt_uw(unsigned &sr, int bit, int &inverted)
-{
-    sr = (sr << 1) | (unsigned)bit;
-    const int xorsum = __popc(sr ^ RT_UWORD);
-    if (xorsum >= 32 - 4) { inverted = 1; return 1; }
-    if (xorsum <= 4) { inverted = 0; return 1; }
-    return 0;
-}
 
 __global__ void __launch_bounds__(64)
 rt_frame_kernel(RtParams rp, const int16_t *__restrict__ soft, const int *__restrict__ soft_count, size_t soft_stride, int vmode)
@@ -72,22 +52,17 @@ rt_frame_kernel(RtParams rp, const int16_t *__restrict__ soft, const int *__rest
         if (s.muw < 100000) s.muw++;
         int gotsync = 0;
         if (rp.oqpsk) {                                                      // :1156-1233
-            s.realimag++; s.realimag %= 2;
             const bool search = (s.cntr > rp.number_of_bits - 68 || s.cntr <= 0 || !s.datacd);
-            int inv;
-            if (s.realimag) { if (search) gotsync = rt_uw(s.sr_imag, bit, s.inv_imag); inv = s.inv_imag; }
-            else { if (search) gotsync = rt_uw(s.sr_real, bit, s.inv_real); inv = s.inv_real; }
-            if (search) { if (!s.gotsync_last) { s.gotsync_last = gotsync; gotsync = 0; } else s.gotsync_last = 0; }
-            else { gotsync = 0; s.gotsync_last = 0; }
+            gotsync = oqpsk_arm_search(s.realimag, s.gotsync_last, s.inv_imag, s.inv_real, search, bit, soft_bit,
+                                       [&](int arm, int b, int &inv) { return uw_phase_invariant<4>(arm ? s.sr_imag : s.sr_real, b, inv); });
             if (gotsync) { if (rp.ifb == 10500 && (abs(s.muw - 80) > 150)) gotsync = 0; }   // :1193-1200
-            if (inv) { bit = 1 - bit; if (soft_bit != 128) soft_bit = 255 - soft_bit; }
         } else {                                                             // :1236-1266
             const int inverted = s.inv_msk;
-            gotsync = rt_uw(s.sr_msk, bit, s.inv_msk);
+            gotsync = uw_phase_invariant<4>(s.sr_msk, bit, s.inv_msk);
             if (s.muw > 250 && gotsync) { if (inverted != s.inv_msk) s.inv_msk = inverted; gotsync = 0; }
-            if (s.inv_msk) { bit = 1 - bit; if (soft_bit != 128) soft_bit = 255 - soft_bit; }
+            if (s.inv_msk) invert_soft(bit, soft_bit);
         }
-        if (s.cntr < 1000000000) s.cntr++;
+        if (s.cntr < CNTR_IDLE) s.cntr++;
         if (s.cntr < 16) {                                                   // :1275-1300
             if (s.cntr == 0) {
                 s.cntr = 16;
@@ -104,27 +79,11 @@ rt_frame_kernel(RtParams rp, const int16_t *__restrict__ soft, const int *__rest
             if (fill < RT_BLOCK) { blocks[(size_t)cur * RT_BLOCK + fill] = (uint8_t)soft_bit; fill++; }
         }
         if (gotsync) { s.cntr = -1; s.datacd = 1; s.datacdcountdown = 12; }  // :1990-2011
-        if (s.cntr + 1 == rp.total_number_of_bits) { s.cntr = 1000000000; s.datacd = 0; s.datacdcountdown = 0; if (vmode) skipping = true; }   // :2013-2029
+        if (s.cntr + 1 == rp.total_number_of_bits) { lost_signal(s); if (vmode) skipping = true; }   // burst time-out :2013-2029
     }
     slots[cur].fill = fill;
     s.slot_cur = cur;
     rp.state[ch] = s;
-}
-
-// AeroLcrc16::calcusingbitsandcheck (aerol.h:287-313) over descrambled bits
-__device__ __forceinline__ bool rt_crc_ok(const uint8_t *bits, int numberofbits)
-{
-    unsigned crc_rec = 0;
-    for (int i = numberofbits - 1; i >= numberofbits - 16; i--) { crc_rec <<= 1; crc_rec |= bits[i]; }
-    numberofbits -= 16;
-    unsigned crc = 0xFFFF;
-    for (int i = 0; i < numberofbits; i++) {
-        const unsigned crc_bit = crc & 1u;
-        crc >>= 1;
-        if (crc_bit ^ bits[i]) crc ^= 0x8408u;
-    }
-    crc = (~crc) & 0xFFFFu;
-    return crc_rec == crc;
 }
 
 __global__ void __launch_bounds__(128)
@@ -166,22 +125,22 @@ rt_trial_kernel(RtParams rp, int smem_per_warp, int sbuf_bytes)
                 __syncwarp();
                 viterbi_decode_warp(sbuf, sets, hist, obits, rc, lane);
                 __syncwarp();
-                for (int k = lane; k < sets; k += 32) obits[k] ^= c_rt_scr[k];            // scrambler.reset(); scrambler.update(deconvol)
+                for (int k = lane; k < sets; k += 32) obits[k] ^= c_scr[k];            // scrambler.reset(); scrambler.update(deconvol)
                 __syncwarp();
                 trials++;
                 int result = RT_NOTHING, nsus = 0, nbytes = 0;
                 if (bp == 64 * 5) {                                                       // R packet test
                     if (!rp.oqpsk) { sl.targetSUSize = 0; sl.targetBlocks = 0; }
-                    const bool ok = rt_crc_ok(obits, 8 * 19);                             // every lane computes the same value
+                    const bool ok = crc16_bits_ok(obits, 8 * 19);                             // every lane computes the same value
                     if (ok) { result = RT_OK_R; nbytes = 19; }
                     else if (rp.oqpsk) result = RT_TEST_FAILED;
                 } else {
-                    const bool hdr = rt_crc_ok(obits, 8 * 6);
+                    const bool hdr = crc16_bits_ok(obits, 8 * 6);
                     if (rp.oqpsk) {                                                       // aerol.h:822-877
                         if (!hdr) result = (bp >= RT_BLOCK) ? RT_BAD : RT_TEST_FAILED;
                         else {
                             nsus = 1 + (bp - 64 * 5) / (64 * 3);
-                            const bool mine = (lane < nsus) ? rt_crc_ok(obits + 8 * 6 + 8 * 12 * lane, 8 * 12) : true;
+                            const bool mine = (lane < nsus) ? crc16_bits_ok(obits + 8 * 6 + 8 * 12 * lane, 8 * 12) : true;
                             const bool all_ok = __all_sync(0xffffffffu, mine);
                             if (!all_ok) result = (bp >= RT_BLOCK) ? RT_BAD : RT_TEST_FAILED;
                             else { result = RT_OK_T; nbytes = sets / 8 - 1; }             // packintobytes(); chop(1)
@@ -236,23 +195,13 @@ rt_trial_kernel(RtParams rp, int smem_per_warp, int sbuf_bytes)
     (void)cur;
 }
 
-__global__ void rt_tick_kernel(RtParams rp)                    // AeroL::updateDCD (aerol.cpp:1109-1122)
-{
-    const int ch = blockIdx.x * blockDim.x + threadIdx.x;
-    if (ch >= rp.n_channels) return;
-    RtState &s = rp.state[ch];
-    if (s.datacdcountdown > 0) s.datacdcountdown -= 3;
-    else { if (s.datacdcountdown < 0) s.datacdcountdown = 0; }
-    if (s.datacd && !s.datacdcountdown) s.datacd = 0;
-}
-
 __global__ void rt_init_kernel(RtParams rp)
 {
     const int ch = blockIdx.x * blockDim.x + threadIdx.x;
     if (ch >= rp.n_channels) return;
     RtState s;
     memset(&s, 0, sizeof s);
-    s.cntr = 1000000000;                                       // AeroL ctor (aerol.cpp:907,927)
+    s.cntr = CNTR_IDLE;                                        // AeroL ctor (aerol.cpp:907,927)
     s.lastpacketstate = RT_NOTHING;
     s.n_open = 1;                                              // the block the RT object starts with
     rp.state[ch] = s;
@@ -261,31 +210,7 @@ __global__ void rt_init_kernel(RtParams rp)
     RtSlot ns; ns.fill = 0; ns.next_trial = rp.oqpsk ? 64 * 2 : 64 * 5; ns.done = 0; ns.closed = 0; ns.targetSUSize = 0; ns.targetBlocks = 0; ns.start_bit = 0;
     rp.slots[(size_t)ch * RT_SLOTS] = ns;
 }
-__global__ void rt_out_reset_kernel(RtParams rp)
-{
-    const int ch = blockIdx.x * blockDim.x + threadIdx.x;
-    if (ch >= rp.n_channels) return;
-    rp.state[ch].out_count = 0;
-}
 
-int rt_init(const RtParams &rp, cudaStream_t st)
-{
-    rt_init_kernel<<<(rp.n_channels + 127) / 128, 128, 0, st>>>(rp);
-    JB_CUDA(cudaGetLastError());
-    return 0;
-}
-int rt_tick(const RtParams &rp, cudaStream_t st)
-{
-    rt_tick_kernel<<<(rp.n_channels + 127) / 128, 128, 0, st>>>(rp);
-    JB_CUDA(cudaGetLastError());
-    return 0;
-}
-int rt_out_reset(const RtParams &rp, cudaStream_t st)
-{
-    rt_out_reset_kernel<<<(rp.n_channels + 127) / 128, 128, 0, st>>>(rp);
-    JB_CUDA(cudaGetLastError());
-    return 0;
-}
 int rt_process(const RtParams &rp, const int16_t *d_soft, const int *d_soft_count, size_t soft_stride, cudaStream_t st, long long *launches, int vmode)
 {
     rt_frame_kernel<<<(rp.n_channels + 63) / 64, 64, 0, st>>>(rp, d_soft, d_soft_count, soft_stride, vmode);
