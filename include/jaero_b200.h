@@ -420,6 +420,45 @@ int jaero_ddc_set_audio_freq(jaero_ddc *d, int channel, double hz);
 int jaero_ddc_get_stats(jaero_ddc *d, int64_t *inputs, int64_t *clipped);
 int64_t jaero_ddc_launch_count(const jaero_ddc *d);
 
+/* ---- PCM rate converter ----
+ * Brings int16 PCM recorded at another audio rate (44100 Hz, say) to the demodulators' rate (Fs 48000) on the device, so that no
+ * CPU resampler sits in front of jaero_batch_write_device / jaero_burst_write_device.
+ *   Input: n_channels independent int16 PCM streams at input_rate, channel-major with a row stride as jaero_batch_write takes
+ *   them; channel c's samples are x_c[n], counted from create, with x_c[n<0] = 0.
+ *   Rates: whole hertz. L / M = output_rate / input_rate, reduced to lowest terms here; rejected when L = M = 1, L > 1024 or
+ *   M > 1024. (8000, 11025, 12000, 16000, 22050, 24000, 32000, 44100, 88200, 96000 and 192000 Hz into 48000, 24000 or 12000 Hz
+ *   all fit; 11025 -> 48000 Hz is L = 640.)
+ *   Filter: one real Kaiser low-pass prototype h of K taps at L * input_rate, summing to L (unit gain at DC). It passes
+ *   [0, passband_hz] within +-0.1 dB and attenuates [min(input_rate, output_rate)/2, L * input_rate/2] by at least 70 dB (designed
+ *   for 76 dB), one stopband for the aliases of the decimation and the images of the x L zero-stuffing. Rejected when
+ *   passband_hz >= min(input_rate, output_rate)/2 or when the design needs more than 2^17 taps.
+ *   Output, per channel c:
+ *     w_c[i] = x_c[i / L] if L divides i, else 0;   v_c[m] = sum_k h[k] w_c[m M - k]
+ *     pcm_c[m] = clamp(rint(v_c[m]), -32768, 32767)  (rint: half to even); clamped samples are counted per channel.
+ *   Output m exists once input floor(m M / L) has arrived: N inputs give ceil(N L / M) outputs per channel. The output does not
+ *   depend on how the stream is cut into writes. A write of 0 samples queues nothing and its output is empty. Sample positions
+ *   are 64-bit. */
+typedef struct jaero_resample jaero_resample;
+/* Host only, no device needed: stages = {L, M, K}; h [K] receives the prototype unless NULL (pass NULL to query K first). */
+int jaero_resample_plan(double input_rate, double output_rate, double passband_hz, int32_t stages[3], double *h);
+/* n_channels streams at input_rate -> output_rate. Fails with JAERO_E_CUDA without a device. */
+int jaero_resample_create(double input_rate, double output_rate, int n_channels, double passband_hz, int device_ordinal, jaero_resample **out);
+void jaero_resample_destroy(jaero_resample *s);
+/* n_samples per channel, pcm[ch * channel_stride + i], channel_stride >= n_samples. HOST pcm (copied before the call returns) */
+int jaero_resample_write(jaero_resample *s, const int16_t *pcm, size_t n_samples, size_t channel_stride);
+/* Same, pcm resident in this GPU's memory */
+int jaero_resample_write_device(jaero_resample *s, const int16_t *d_pcm, size_t n_samples, size_t channel_stride);
+/* The PCM the last write produced: d_pcm[ch * stride + i], i < n, device memory, rows 16-byte aligned (stride a multiple of 8).
+ * Valid until the next write and ordered on the resampler's stream: put the consuming batch on the same stream. */
+int jaero_resample_output(jaero_resample *s, const int16_t **d_pcm, size_t *n, size_t *stride);
+/* Host copy of the same: out[ch * cap_per_channel + i]; *n = outputs per channel. Synchronises. */
+int jaero_resample_read_pcm(jaero_resample *s, int16_t *out, size_t cap_per_channel, size_t *n);
+/* Run on a caller-owned CUDA stream (cudaStream_t as void*; NULL = back to the resampler's own stream) */
+int jaero_resample_set_stream(jaero_resample *s, void *cuda_stream);
+/* input samples per channel written so far; clipped [n_channels] output samples clamped to the int16 range (either may be NULL) */
+int jaero_resample_get_stats(jaero_resample *s, int64_t *inputs, int64_t *clipped);
+int64_t jaero_resample_launch_count(const jaero_resample *s);
+
 /* ---- wideband carrier scanner ----
  * Finds the carriers in the IQ stream the down-converter takes, so that its channels can be planned from the stream itself.
  * The scanner averages the stream's power spectrum on the device; jaero_scan_find_carriers (host only) finds and measures the

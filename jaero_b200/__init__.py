@@ -72,6 +72,9 @@ EXPORTS = ["jaero_last_error", "jaero_device_count", "jaero_batch_create", "jaer
            "jaero_ddc_plan", "jaero_ddc_create", "jaero_ddc_destroy", "jaero_ddc_write", "jaero_ddc_write_device", "jaero_ddc_output",
            "jaero_ddc_read_pcm", "jaero_ddc_set_stream", "jaero_ddc_set_offset", "jaero_ddc_set_audio_freq", "jaero_ddc_get_stats",
            "jaero_ddc_launch_count", "jaero_ddc_plan_rational", "jaero_ddc_create_rational",
+           "jaero_resample_plan", "jaero_resample_create", "jaero_resample_destroy", "jaero_resample_write", "jaero_resample_write_device",
+           "jaero_resample_output", "jaero_resample_read_pcm", "jaero_resample_set_stream", "jaero_resample_get_stats",
+           "jaero_resample_launch_count",
            "jaero_scan_create", "jaero_scan_destroy", "jaero_scan_write", "jaero_scan_write_device", "jaero_scan_set_stream",
            "jaero_scan_reset", "jaero_scan_read", "jaero_scan_launch_count", "jaero_scan_find_carriers"]
 MODES = {0: "unknown", 1: "msk600", 2: "msk1200", 3: "oqpsk8400", 4: "oqpsk10500"}
@@ -196,6 +199,15 @@ def lib():
         L.jaero_ddc_set_offset.argtypes = [vp, i, d]; L.jaero_ddc_set_audio_freq.argtypes = [vp, i, d]
         L.jaero_ddc_get_stats.argtypes = [vp, vp, vp]
         L.jaero_ddc_launch_count.argtypes = [vp]; L.jaero_ddc_launch_count.restype = ctypes.c_int64
+        L.jaero_resample_plan.argtypes = [d, d, d, vp, vp]
+        L.jaero_resample_create.argtypes = [d, d, i, d, i, ctypes.POINTER(vp)]
+        L.jaero_resample_destroy.argtypes = [vp]; L.jaero_resample_destroy.restype = None
+        L.jaero_resample_write.argtypes = [vp, vp, sz, sz]; L.jaero_resample_write_device.argtypes = [vp, vp, sz, sz]
+        L.jaero_resample_output.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(sz), ctypes.POINTER(sz)]
+        L.jaero_resample_read_pcm.argtypes = [vp, vp, sz, ctypes.POINTER(sz)]
+        L.jaero_resample_set_stream.argtypes = [vp, vp]
+        L.jaero_resample_get_stats.argtypes = [vp, vp, vp]
+        L.jaero_resample_launch_count.argtypes = [vp]; L.jaero_resample_launch_count.restype = ctypes.c_int64
         L.jaero_scan_create.argtypes = [d, i, i, i, ctypes.POINTER(vp)]
         L.jaero_scan_destroy.argtypes = [vp]; L.jaero_scan_destroy.restype = None
         L.jaero_scan_write.argtypes = [vp, vp, sz, i]; L.jaero_scan_write_device.argtypes = [vp, vp, sz, i]
@@ -955,6 +967,85 @@ class Ddc:
     def close(self):
         if self.h:
             lib().jaero_ddc_destroy(self.h); self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def resample_plan(input_rate, output_rate, passband_hz):
+    """The rate converter's filter for a set-up (host only, no device): dict(L, M, K, h), output_rate / input_rate = L / M reduced
+    to lowest terms, h the K-tap low-pass prototype at L * input_rate, summing to L."""
+    st = np.zeros(3, dtype=np.int32)
+    args = (float(input_rate), float(output_rate), float(passband_hz), _p(st))
+    _check(lib().jaero_resample_plan(*args, None))
+    h = np.zeros(int(st[2]))
+    _check(lib().jaero_resample_plan(*args, _p(h)))
+    return dict(L=int(st[0]), M=int(st[1]), K=int(st[2]), h=h)
+
+
+class Resampler:
+    """PCM rate converter (include/jaero_b200.h, jaero_resample_*): n_channels int16 PCM streams at input_rate -> int16 PCM at
+    output_rate (the demodulators' 48 kHz by default), on the device. passband_hz defaults to 0.45 min(input_rate, output_rate)."""
+
+    def __init__(self, input_rate, n_channels, output_rate=48000, passband_hz=None, device=0):
+        if n_channels <= 0:
+            raise JaeroError("n_channels must be positive")
+        if passband_hz is None:
+            passband_hz = 0.45 * min(float(input_rate), float(output_rate))
+        self.n = int(n_channels)
+        self.input_rate, self.output_rate, self.passband_hz = float(input_rate), float(output_rate), float(passband_hz)
+        self.h = ctypes.c_void_p()
+        _check(lib().jaero_resample_create(self.input_rate, self.output_rate, self.n, self.passband_hz, device, ctypes.byref(self.h)))
+        self.plan = resample_plan(input_rate, output_rate, passband_hz)
+
+    def write(self, pcm):
+        """pcm: int16 array [n_channels, n_samples] (host); rows may be strided"""
+        pcm = np.asarray(pcm)
+        if pcm.dtype != np.int16 or pcm.ndim != 2 or pcm.shape[0] != self.n:
+            raise ValueError("pcm must be int16 [%d, n_samples]" % self.n)
+        if pcm.strides[1] != 2 or pcm.strides[0] % 2:
+            pcm = np.ascontiguousarray(pcm)
+        stride = pcm.strides[0] // 2 if pcm.shape[0] > 1 else pcm.shape[1]
+        _check(lib().jaero_resample_write(self.h, _p(pcm), pcm.shape[1], stride))
+
+    def write_device(self, dev_ptr, n_samples, stride):
+        """the same from a DEVICE buffer [n_channels][stride] int16"""
+        _check(lib().jaero_resample_write_device(self.h, ctypes.c_void_p(dev_ptr), int(n_samples), int(stride)))
+
+    def output(self):
+        """(device pointer, outputs per channel, row stride) of the PCM the last write produced"""
+        a, n, s = ctypes.c_void_p(), ctypes.c_size_t(), ctypes.c_size_t()
+        _check(lib().jaero_resample_output(self.h, ctypes.byref(a), ctypes.byref(n), ctypes.byref(s)))
+        return a.value, n.value, s.value
+
+    def read_pcm(self):
+        """host copy [n_channels, n] of the PCM the last write produced"""
+        _, n, _ = self.output()
+        out = np.zeros((self.n, max(n, 1)), dtype=np.int16)
+        got = ctypes.c_size_t()
+        _check(lib().jaero_resample_read_pcm(self.h, _p(out), out.shape[1], ctypes.byref(got)))
+        return out[:, :got.value]
+
+    def set_stream(self, cuda_stream):
+        _check(lib().jaero_resample_set_stream(self.h, ctypes.c_void_p(cuda_stream)))
+
+    def stats(self):
+        """(input samples per channel written, clipped output samples per channel)"""
+        n = ctypes.c_int64()
+        clipped = np.zeros(self.n, dtype=np.int64)
+        _check(lib().jaero_resample_get_stats(self.h, ctypes.byref(n), _p(clipped)))
+        return n.value, clipped
+
+    @property
+    def launches(self):
+        return lib().jaero_resample_launch_count(self.h)
+
+    def close(self):
+        if self.h:
+            lib().jaero_resample_destroy(self.h); self.h = None
 
     def __del__(self):
         try:

@@ -18,6 +18,7 @@ UNITS = [
     ("frame_layers.cu", []),
     ("reassembly.cu", []),
     ("ddc.cu", []),
+    ("resample.cu", []),
     ("scan.cu", []),
     ("prefilter.cu", ["-fmad=false"]),
     ("fastfir.cu", ["-fmad=false"]),

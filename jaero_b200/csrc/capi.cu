@@ -12,6 +12,7 @@
 #include "frame_layers.cuh"
 #include "ddc.cuh"
 #include "scan.cuh"
+#include "resample.cuh"
 #include <cstring>
 #include <complex>
 #include <climits>
@@ -2103,11 +2104,12 @@ int jaero_ingest_flush(jaero_ingest *g, jaero_batch *b, size_t n)
 static const double DDC_DESIGN_DB = 76.0;
 static const int DDC_MAX_TAPS = 1 << 15;
 
-static int kaiser_length(double fs, double fpass, double fstop)
+// Taps for the design; max_taps + 1 when the estimate reaches max_taps
+static int kaiser_length(double fs, double fpass, double fstop, int max_taps = DDC_MAX_TAPS)
 {
     const double dw = 2 * M_PI * (fstop - fpass) / fs;
     const double n = (DDC_DESIGN_DB - 7.95) / (2.285 * dw) + 1.0;
-    if (!(n < DDC_MAX_TAPS)) return DDC_MAX_TAPS + 1;
+    if (!(n < max_taps)) return max_taps + 1;
     return (int)ceil(n) | 1;                                        // odd: a whole-sample group delay
 }
 static double bessel_i0(double x)
@@ -2410,6 +2412,183 @@ int jaero_ddc_get_stats(jaero_ddc *d, int64_t *inputs, int64_t *clipped)
         JB_CUDA(cudaSetDevice(d->device));
         JB_CUDA(cudaMemcpyAsync(clipped, d->p.clipped, d->p.n_channels * sizeof(int64_t), cudaMemcpyDeviceToHost, d->stream));
         JB_CUDA(cudaStreamSynchronize(d->stream));
+    }
+    return JAERO_OK;
+}
+
+} // extern "C"
+
+// ------------------------------------------------------------------ PCM rate converter
+// One Kaiser low-pass prototype at L * input_rate, designed as the down-converter's stages are: it passes [0, passband_hz] and
+// stops from min(input_rate, output_rate)/2, which removes both the aliases of the decimation and the images of the x L
+// zero-stuffing. 11025 -> 48000 Hz is L = 640 and about 61000 taps, hence limits above the down-converter's.
+static const int RESAMPLE_MAX_RATIO = 1024;
+static const int RESAMPLE_MAX_TAPS = 1 << 17;
+
+struct ResamplePlan { int L, M, K; double fs_up, fpass, fstop; };
+
+static int resample_plan_stages(double fs_in, double fs_out, double passband, ResamplePlan *out, const char *fn)
+{
+    const std::string f(fn);
+    for (double r : {fs_in, fs_out})
+        if (!(std::isfinite(r) && r >= 1 && r <= 2147483647.0 && r == floor(r))) { set_error(f + ": rates must be positive whole hertz"); return JAERO_E_ARG; }
+    const long long a = (long long)fs_in, b = (long long)fs_out, g = std::gcd(a, b);
+    const long long L = b / g, M = a / g;
+    if (L == 1 && M == 1) { set_error(f + ": input and output rates are equal; there is nothing to resample"); return JAERO_E_ARG; }
+    if (L > RESAMPLE_MAX_RATIO || M > RESAMPLE_MAX_RATIO) {
+        set_error(f + ": output_rate/input_rate reduces to " + std::to_string(L) + "/" + std::to_string(M) + "; L and M must not exceed " +
+                  std::to_string(RESAMPLE_MAX_RATIO));
+        return JAERO_E_ARG;
+    }
+    const double fstop = 0.5 * (double)std::min(a, b);
+    if (!(passband > 0 && passband < fstop)) { set_error(f + ": passband_hz must lie in (0, min(input_rate, output_rate)/2)"); return JAERO_E_ARG; }
+    ResamplePlan c{(int)L, (int)M, 0, (double)L * fs_in, passband, fstop};
+    c.K = kaiser_length(c.fs_up, passband, fstop, RESAMPLE_MAX_TAPS);
+    if (c.K > RESAMPLE_MAX_TAPS) {
+        set_error(f + ": the filter would need more than " + std::to_string(RESAMPLE_MAX_TAPS) + " taps; lower passband_hz"); return JAERO_E_ARG; }
+    *out = c;
+    return JAERO_OK;
+}
+// h sums to L: the zero-stuffing divides the signal's level by L, so the passband gain is 1.
+static void resample_design(const ResamplePlan &c, double *h)
+{
+    kaiser_lowpass(c.fs_up, c.fpass, c.fstop, c.K, h);
+    for (int k = 0; k < c.K; k++) h[k] *= c.L;
+}
+
+struct jaero_resample {
+    int device; cudaStream_t stream, own_stream;
+    std::vector<void *> allocs;
+    ResampleParams p;
+    long long n_in, launches;                                        // samples per channel written so far
+    int16_t *d_in; size_t in_cap;                                    // host writes: the PCM staged on the device, [C][n]
+    double *d_x; size_t x_cap;                                       // [H + n][cpad] rows of the current write
+    int16_t *d_pcm; size_t pcm_cap, pcm_n, pcm_stride;
+};
+
+extern "C" {
+
+int jaero_resample_plan(double input_rate, double output_rate, double passband_hz, int32_t stages[3], double *h)
+{
+    if (!stages) { set_error("jaero_resample_plan: null argument"); return JAERO_E_ARG; }
+    ResamplePlan c;
+    const int r = resample_plan_stages(input_rate, output_rate, passband_hz, &c, "jaero_resample_plan");
+    if (r) return r;
+    stages[0] = c.L; stages[1] = c.M; stages[2] = c.K;
+    if (h) resample_design(c, h);
+    return JAERO_OK;
+}
+
+int jaero_resample_create(double input_rate, double output_rate, int n_channels, double passband_hz, int device, jaero_resample **out)
+{
+    const char *fn = "jaero_resample_create";
+    if (!out || n_channels <= 0) { set_error(std::string(fn) + ": bad argument"); return JAERO_E_ARG; }
+    ResamplePlan c;
+    { const int r = resample_plan_stages(input_rate, output_rate, passband_hz, &c, fn); if (r) return r; }
+    CreateGuard<jaero_resample> guard(jaero_resample_destroy);
+    { const int e = guard.begin(fn, device); if (e) return e; }
+    jaero_resample *s = guard.obj;
+    s->own_stream = s->stream;
+    ResampleParams &p = s->p;
+    p.n_channels = n_channels; p.cpad = (n_channels + 31) & ~31;
+    p.L = c.L; p.M = c.M; p.K = c.K;
+    p.R = (c.K + c.L - 1) / c.L;
+    p.H = p.R;                                                       // the first output of a write reads back R - 1 rows
+    std::vector<double> h(c.K), hp((size_t)c.L * p.R, 0.0);           // [L][R] per-phase taps, hp[phi][r] = h[phi + r L]
+    resample_design(c, h.data());
+    for (int k = 0; k < c.K; k++) hp[(size_t)(k % c.L) * p.R + k / c.L] = h[k];
+    double *dhp;
+    int rc = 0;
+    rc |= owned_alloc(s, &dhp, hp.size());
+    rc |= owned_alloc(s, &p.hist, (size_t)p.H * p.cpad);
+    rc |= owned_alloc(s, &p.clipped, (size_t)p.cpad);
+    if (rc) return JAERO_E_CUDA;
+    p.hp = dhp;
+    JB_CUDA(cudaMemcpyAsync(dhp, hp.data(), hp.size() * sizeof(double), cudaMemcpyHostToDevice, s->stream));
+    JB_CUDA(cudaStreamSynchronize(s->stream));                       // the zeroed history and the table are in place
+    *out = guard.release();
+    return JAERO_OK;
+}
+void jaero_resample_destroy(jaero_resample *s)
+{
+    if (!s) return;
+    cudaSetDevice(s->device);
+    cudaStreamSynchronize(s->stream);
+    release(s, {s->d_in, s->d_x, s->d_pcm}, {}, s->own_stream);
+}
+int64_t jaero_resample_launch_count(const jaero_resample *s) { return s ? s->launches : 0; }
+
+int jaero_resample_write_device(jaero_resample *s, const int16_t *d_pcm, size_t n, size_t stride)
+{
+    if (!s || !d_pcm) { set_error("jaero_resample_write_device: null argument"); return JAERO_E_ARG; }
+    if ((uintptr_t)d_pcm & 1) { set_error("jaero_resample_write_device: PCM pointer not aligned to one sample"); return JAERO_E_ARG; }
+    if (stride < n) { set_error("jaero_resample_write_device: channel stride is smaller than n_samples"); return JAERO_E_ARG; }
+    if (n > ((size_t)1 << 34)) { set_error("jaero_resample_write_device: too many samples in one write"); return JAERO_E_ARG; }
+    JB_CUDA(cudaSetDevice(s->device));
+    const ResampleParams &p = s->p;
+    const long long n0 = s->n_in;
+    // outputs m with floor(m M / L) in [n0, n0 + n): ceil((n0 + n) L / M) - ceil(n0 L / M)
+    const size_t M_out = (size_t)(((n0 + (long long)n) * p.L + p.M - 1) / p.M - (n0 * p.L + p.M - 1) / p.M);
+    const size_t out_stride = std::max<size_t>(8, (M_out + 7) & ~(size_t)7);   // 16-byte rows: jaero_batch_write_device reads them in place
+    if (n > 0) {
+        // a failed write leaves the output of the previous one described
+        if (grow(&s->d_x, &s->x_cap, ((size_t)p.H + n) * p.cpad, s->stream) ||
+            grow(&s->d_pcm, &s->pcm_cap, (size_t)p.n_channels * out_stride, s->stream)) return JAERO_E_CUDA;
+        if (resample_run(p, d_pcm, stride, n0, (long long)n, s->d_x, s->d_pcm, out_stride, s->stream, &s->launches)) return JAERO_E_CUDA;
+        s->n_in += (long long)n;
+    }
+    s->pcm_n = M_out; s->pcm_stride = out_stride;
+    return JAERO_OK;
+}
+int jaero_resample_write(jaero_resample *s, const int16_t *pcm, size_t n, size_t stride)
+{
+    if (!s || !pcm) { set_error("jaero_resample_write: null argument"); return JAERO_E_ARG; }
+    if (stride < n) { set_error("jaero_resample_write: channel stride is smaller than n_samples"); return JAERO_E_ARG; }
+    if (n > ((size_t)1 << 34)) { set_error("jaero_resample_write: too many samples in one write"); return JAERO_E_ARG; }
+    JB_CUDA(cudaSetDevice(s->device));
+    const size_t C = (size_t)s->p.n_channels;
+    if (grow(&s->d_in, &s->in_cap, std::max<size_t>(C * n, 1), s->stream)) return JAERO_E_CUDA;
+    if (n) {
+        JB_CUDA(cudaMemcpy2DAsync(s->d_in, n * sizeof(int16_t), pcm, stride * sizeof(int16_t), n * sizeof(int16_t), C, cudaMemcpyHostToDevice,
+                                  s->stream));
+        JB_CUDA(cudaStreamSynchronize(s->stream));                   // the caller may reuse its pageable buffer on return
+    }
+    return jaero_resample_write_device(s, s->d_in, n, n);
+}
+int jaero_resample_output(jaero_resample *s, const int16_t **d_pcm, size_t *n, size_t *stride)
+{
+    if (!s || !d_pcm || !n || !stride) { set_error("jaero_resample_output: null argument"); return JAERO_E_ARG; }
+    *d_pcm = s->d_pcm; *n = s->pcm_n; *stride = s->pcm_stride;
+    return JAERO_OK;
+}
+int jaero_resample_read_pcm(jaero_resample *s, int16_t *out, size_t cap, size_t *n)
+{
+    if (!s || !out || !n) { set_error("jaero_resample_read_pcm: null argument"); return JAERO_E_ARG; }
+    if (cap < s->pcm_n) { set_error("jaero_resample_read_pcm: cap_per_channel is smaller than the last write's output"); return JAERO_E_ARG; }
+    JB_CUDA(cudaSetDevice(s->device));
+    if (s->pcm_n)
+        JB_CUDA(cudaMemcpy2DAsync(out, cap * sizeof(int16_t), s->d_pcm, s->pcm_stride * sizeof(int16_t), s->pcm_n * sizeof(int16_t),
+                                  s->p.n_channels, cudaMemcpyDeviceToHost, s->stream));
+    JB_CUDA(cudaStreamSynchronize(s->stream));
+    *n = s->pcm_n;
+    return JAERO_OK;
+}
+int jaero_resample_set_stream(jaero_resample *s, void *cuda_stream)
+{
+    if (!s) { set_error("null handle"); return JAERO_E_ARG; }
+    JB_CUDA(cudaSetDevice(s->device));
+    JB_CUDA(cudaStreamSynchronize(s->stream));
+    s->stream = cuda_stream ? (cudaStream_t)cuda_stream : s->own_stream;
+    return JAERO_OK;
+}
+int jaero_resample_get_stats(jaero_resample *s, int64_t *inputs, int64_t *clipped)
+{
+    if (!s) { set_error("null handle"); return JAERO_E_ARG; }
+    if (inputs) *inputs = s->n_in;
+    if (clipped) {
+        JB_CUDA(cudaSetDevice(s->device));
+        JB_CUDA(cudaMemcpyAsync(clipped, s->p.clipped, s->p.n_channels * sizeof(int64_t), cudaMemcpyDeviceToHost, s->stream));
+        JB_CUDA(cudaStreamSynchronize(s->stream));
     }
     return JAERO_OK;
 }
