@@ -528,6 +528,73 @@ typedef struct jaero_carrier {
 int jaero_scan_find_carriers(const double *psd, int nfft, double input_rate, const jaero_scan_params *params,
                              jaero_carrier *out, int cap, int *n_found);
 
+/* ---- mode identifier ----
+ * Tells each PCM channel's JAERO bit rate and carrier frequency from the spectral lines of its square. Squaring an MSK or OQPSK
+ * carrier at fc leaves two discrete lines at 2 fc +- fb / 2: their distance is the bit rate and their midpoint twice the carrier
+ * (the physics of the reference's CoarseFreqEstimate, searched here at every JAERO rate over the whole band). The identifier
+ * averages the squared signal's power spectrum on the device; jaero_ident_classify (host only) finds the line pair in it.
+ * Spectrum contract, per channel c of n_channels int16 PCM streams at Fs (channel-major with a row stride, as jaero_batch_write
+ * takes them, so down-converter, rate-converter or recording output feeds it directly):
+ *   x_c[n] = pcm_c[n] / 32768, counted from create or the last reset. N = nfft, hop = N / 2; frame f is x_c[f hop + n], n < N,
+ *   and counts once its last sample has arrived. w[n] = 0.5 - 0.5 cos(2 pi n / N) (periodic Hann). Per frame:
+ *     X[k] = sum_n w[n] x_c[f hop + n] exp(-2 pi i k n / N)
+ *     A[k] = 2 X[k] for 0 < k < N/2, else 0                  (the analytic signal, without its DC and Nyquist bins)
+ *     a[n] = (1/N) sum_k A[k] exp(+2 pi i k n / N)
+ *     Y[k] = sum_n a[n]^2 exp(-2 pi i k n / N)
+ *   sq_mean_c[i] = (1/F) sum_f |Y_f[k]|^2 / (sum_n w[n]^2)^2 over the F frames so far, in fftshift order: index i is bin
+ *   k = (i + N/2) mod N, at (i - N/2) Fs / N Hz of the squared signal, twice the PCM frequency modulo Fs. A unit cosine at a bin
+ *   centre gives 1 at its 2f bin. Frames are added in frame order, so sq_mean is bit-identical however the stream is cut into
+ *   writes and whatever the batch's channel count and order. With no frame yet it is 0.
+ * Limits: Fs whole hertz in [8000, 192000]; nfft a power of two from 2^10 to 2^14; anything else is JAERO_E_ARG. */
+typedef struct jaero_ident jaero_ident;
+/* Fails with JAERO_E_CUDA without a device. */
+int jaero_ident_create(double Fs, int n_channels, int nfft, int device_ordinal, jaero_ident **out);
+void jaero_ident_destroy(jaero_ident *d);
+/* n_samples per channel, pcm[ch * channel_stride + i], channel_stride >= n_samples. HOST pcm (copied before the call returns).
+ * A failed write leaves the average unchanged. */
+int jaero_ident_write(jaero_ident *d, const int16_t *pcm, size_t n_samples, size_t channel_stride);
+/* Same, pcm resident in this GPU's memory (aligned to one sample), e.g. jaero_ddc_output's on the same stream */
+int jaero_ident_write_device(jaero_ident *d, const int16_t *d_pcm, size_t n_samples, size_t channel_stride);
+/* Run on a caller-owned CUDA stream (cudaStream_t as void*; NULL = back to the identifier's own stream) */
+int jaero_ident_set_stream(jaero_ident *d, void *cuda_stream);
+/* Start a new average: the frame count, the sample origin and sq_mean restart */
+int jaero_ident_reset(jaero_ident *d);
+/* sq_mean [n_channels][nfft] (may be NULL), *frames = frames averaged per channel (may be NULL). Synchronises. */
+int jaero_ident_read(jaero_ident *d, double *sq_mean, int64_t *frames);
+int64_t jaero_ident_launch_count(const jaero_ident *d);
+
+/* Classification, host only (no device), of one channel's sq_mean (nfft and Fs as for create, values finite and >= 0).
+ * params NULL: the defaults {5 dB, 400 Hz, 0.5}. 5 dB lies between the
+ * largest score of noise (about 3 dB over 4 s) and the weakest right rate at Eb/N0 4 dB (600 bps, about 6.5 dB).
+ *   floor: jaero_scan_find_carriers' sliding order statistic with floor_window_hz and floor_quantile, bin_hz = Fs / nfft.
+ *   Q[i] = sq_mean[i] / floor[i], 0 where floor[i] is 0.
+ *   For each mode m in (MSK600, MSK1200, OQPSK8400, OQPSK10500), fb_m = 600, 1200, 8400, 10500, D_m = round(fb_m nfft / Fs)
+ *   (half away from zero): score_m = max over i of min(Q[i], max over e in (-1, 0, +1) of Q[(i + D_m + e) mod nfft]), the first i
+ *   on ties, and for it the first e with the largest Q; j = i + D_m + e. score_db[m] = 10 log10(score_m) (-HUGE_VAL for 0).
+ *   best = the mode with the largest score (the first on ties); margin_db = score_db[best] - the largest other score_db.
+ *   Each line of best's pair (bins i and j mod nfft) is refined by a log-parabolic fit through its bin and its two neighbours
+ *   (indices mod nfft): delta = (l- - l+) / (2 (l- - 2 l0 + l+)) with l = ln sq_mean, clamped to [-0.5, 0.5]; 0 when any of the
+ *   three values is <= 0 or the denominator is 0. With p = i + delta_i and q = j + delta_j (j unwrapped), bin_hz = Fs / nfft:
+ *     line_hz[0] = (i + delta_i - nfft/2) bin_hz,  line_hz[1] = ((j mod nfft) + delta_j - nfft/2) bin_hz   (squared signal)
+ *     fb_hz = (q - p) bin_hz,  carrier_hz = ((mid mod Fs) + Fs) mod Fs / 2 with mid = ((p + q) / 2 - nfft/2) bin_hz, in [0, Fs/2)
+ *   mode = best if score_db[best] >= threshold_db, else JAERO_MODE_UNKNOWN. frames is 0 here: the classifier sees only the
+ *   spectrum; jaero_ident_read reports the frames behind it. */
+typedef struct jaero_ident_params {
+    double threshold_db;      /* finite */
+    double floor_window_hz;   /* > 0 */
+    double floor_quantile;    /* [0, 1] */
+} jaero_ident_params;
+typedef struct jaero_ident_result {
+    double carrier_hz;        /* PCM frequency of the carrier, [0, Fs/2) */
+    double fb_hz;             /* measured distance between the lines */
+    double line_hz[2];        /* the lines, Hz of the squared signal */
+    double score_db[4];       /* per mode, JAERO_MODE_* - 1 */
+    double margin_db;
+    int64_t frames;
+    int32_t mode;             /* JAERO_MODE_* */
+} jaero_ident_result;
+int jaero_ident_classify(const double *sq_mean, int nfft, double Fs, const jaero_ident_params *params, jaero_ident_result *out);
+
 /* ---- ISU / SSU reassembly and ACARS block parsing (SURVEY.md section 8(f)4, host side) ----
  * One handle per channel. Replaces RISUData::update (JAERO/aerol.cpp:27-112), ISUData::update (:151-214),
  * ParserISU::parse (:340-487) and ACARSDefragmenter (:221-329), fed the way AeroL::Decode feeds them (:1357-1399 R

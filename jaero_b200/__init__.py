@@ -76,7 +76,9 @@ EXPORTS = ["jaero_last_error", "jaero_device_count", "jaero_batch_create", "jaer
            "jaero_resample_output", "jaero_resample_read_pcm", "jaero_resample_set_stream", "jaero_resample_get_stats",
            "jaero_resample_launch_count",
            "jaero_scan_create", "jaero_scan_destroy", "jaero_scan_write", "jaero_scan_write_device", "jaero_scan_set_stream",
-           "jaero_scan_reset", "jaero_scan_read", "jaero_scan_launch_count", "jaero_scan_find_carriers"]
+           "jaero_scan_reset", "jaero_scan_read", "jaero_scan_launch_count", "jaero_scan_find_carriers",
+           "jaero_ident_create", "jaero_ident_destroy", "jaero_ident_write", "jaero_ident_write_device", "jaero_ident_set_stream",
+           "jaero_ident_reset", "jaero_ident_read", "jaero_ident_launch_count", "jaero_ident_classify"]
 MODES = {0: "unknown", 1: "msk600", 2: "msk1200", 3: "oqpsk8400", 4: "oqpsk10500"}
 CARRIER_AT_DC, CARRIER_AT_EDGE = 1, 2
 
@@ -90,6 +92,17 @@ class Carrier(ctypes.Structure):
     """jaero_carrier (include/jaero_b200.h)."""
     _fields_ = [(n, ctypes.c_double) for n in ("center_hz", "peak_hz", "lo_hz", "hi_hz", "width_hz", "power", "snr_db", "peak_db",
                                                 "floor")] + [("mode", ctypes.c_int32), ("flags", ctypes.c_int32)]
+
+
+class IdentParams(ctypes.Structure):
+    """jaero_ident_params (include/jaero_b200.h)."""
+    _fields_ = [(n, ctypes.c_double) for n in ("threshold_db", "floor_window_hz", "floor_quantile")]
+
+
+class IdentResult(ctypes.Structure):
+    """jaero_ident_result (include/jaero_b200.h)."""
+    _fields_ = [("carrier_hz", ctypes.c_double), ("fb_hz", ctypes.c_double), ("line_hz", ctypes.c_double * 2),
+                ("score_db", ctypes.c_double * 4), ("margin_db", ctypes.c_double), ("frames", ctypes.c_int64), ("mode", ctypes.c_int32)]
 
 
 def lib():
@@ -216,6 +229,14 @@ def lib():
         L.jaero_scan_read.argtypes = [vp, vp, vp, vp]
         L.jaero_scan_launch_count.argtypes = [vp]; L.jaero_scan_launch_count.restype = ctypes.c_int64
         L.jaero_scan_find_carriers.argtypes = [vp, i, d, ctypes.POINTER(ScanParams), vp, i, ctypes.POINTER(i)]
+        L.jaero_ident_create.argtypes = [d, i, i, i, ctypes.POINTER(vp)]
+        L.jaero_ident_destroy.argtypes = [vp]; L.jaero_ident_destroy.restype = None
+        L.jaero_ident_write.argtypes = [vp, vp, sz, sz]; L.jaero_ident_write_device.argtypes = [vp, vp, sz, sz]
+        L.jaero_ident_set_stream.argtypes = [vp, vp]
+        L.jaero_ident_reset.argtypes = [vp]
+        L.jaero_ident_read.argtypes = [vp, vp, vp]
+        L.jaero_ident_launch_count.argtypes = [vp]; L.jaero_ident_launch_count.restype = ctypes.c_int64
+        L.jaero_ident_classify.argtypes = [vp, i, d, ctypes.POINTER(IdentParams), ctypes.POINTER(IdentResult)]
         _lib = L
     return _lib
 
@@ -1158,3 +1179,149 @@ def channel_plan(carriers, input_rate, decimation, interpolation=1):
             demod=dict(kind=s["kind"], n_channels=len(group), fb=s["fb"], freq_center=s["audio_hz"], lockingbw=s["lockingbw"]),
             carriers=group)
     return out, unplanned
+
+
+class Identifier:
+    """Mode identifier (include/jaero_b200.h, jaero_ident_*): per channel of n_channels int16 PCM streams at Fs, the averaged power
+    spectrum of the squared analytic signal, nfft bins in fftshift order, frames every nfft // 2 samples. identify() finds the
+    JAERO bit rate and the carrier in one row of it."""
+
+    def __init__(self, Fs, n_channels, nfft=16384, device=0):
+        self.Fs, self.n, self.nfft = float(Fs), int(n_channels), int(nfft)
+        self.h = ctypes.c_void_p()
+        _check(lib().jaero_ident_create(self.Fs, self.n, self.nfft, device, ctypes.byref(self.h)))
+
+    def write(self, pcm):
+        """pcm: int16 array [n_channels, n_samples] (host); rows may be strided"""
+        pcm = np.asarray(pcm)
+        if pcm.dtype != np.int16 or pcm.ndim != 2 or pcm.shape[0] != self.n:
+            raise ValueError("pcm must be int16 [%d, n_samples]" % self.n)
+        if pcm.strides[1] != 2 or pcm.strides[0] % 2:
+            pcm = np.ascontiguousarray(pcm)
+        stride = pcm.strides[0] // 2 if pcm.shape[0] > 1 else pcm.shape[1]
+        _check(lib().jaero_ident_write(self.h, _p(pcm), pcm.shape[1], stride))
+
+    def write_device(self, dev_ptr, n_samples, stride):
+        """the same from a DEVICE buffer [n_channels][stride] int16 (Ddc.output / Resampler.output on the same stream)"""
+        _check(lib().jaero_ident_write_device(self.h, ctypes.c_void_p(dev_ptr), int(n_samples), int(stride)))
+
+    def reset(self):
+        _check(lib().jaero_ident_reset(self.h))
+
+    def read(self):
+        """(sq_mean [n_channels, nfft], frames averaged per channel)"""
+        sq = np.zeros((self.n, self.nfft)); fr = ctypes.c_int64()
+        _check(lib().jaero_ident_read(self.h, _p(sq), ctypes.byref(fr)))
+        return sq, fr.value
+
+    def freqs(self):
+        """frequency of each bin, Hz of the squared signal (twice the PCM frequency, modulo Fs)"""
+        return (np.arange(self.nfft) - self.nfft // 2) * (self.Fs / self.nfft)
+
+    def set_stream(self, cuda_stream):
+        _check(lib().jaero_ident_set_stream(self.h, ctypes.c_void_p(cuda_stream)))
+
+    @property
+    def launches(self):
+        return lib().jaero_ident_launch_count(self.h)
+
+    def close(self):
+        if self.h:
+            lib().jaero_ident_destroy(self.h); self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+IDENT_MODES = ("msk600", "msk1200", "oqpsk8400", "oqpsk10500")     # the order of jaero_ident_result.score_db
+
+
+def identify(sq_mean_row, Fs, frames=0, threshold_db=5.0, floor_window_hz=400.0, floor_quantile=0.5):
+    """The JAERO bit rate and carrier of one Identifier.read row (host only, no device; include/jaero_b200.h,
+    jaero_ident_classify): dict(mode, carrier_hz, fb_hz, line_hz, score_db {mode: dB}, margin_db, frames), mode as a MODES string."""
+    row = np.ascontiguousarray(sq_mean_row, dtype=np.float64)
+    prm = IdentParams(threshold_db, floor_window_hz, floor_quantile)
+    r = IdentResult()
+    _check(lib().jaero_ident_classify(_p(row), len(row), float(Fs), ctypes.byref(prm), ctypes.byref(r)))
+    return dict(mode=MODES[r.mode], carrier_hz=r.carrier_hz, fb_hz=r.fb_hz, line_hz=[r.line_hz[0], r.line_hz[1]],
+                score_db=dict(zip(IDENT_MODES, r.score_db)), margin_db=r.margin_db, frames=int(frames))
+
+
+# The probe's down-converter: every candidate at 12 kHz of 48 kHz audio, 16 kHz wide, so that a 10.5 kbps carrier up to a few
+# kilohertz off its measured centre still lies inside the channel and its square's lines below Fs / 2.
+PROBE_AUDIO_HZ, PROBE_BANDWIDTH, PROBE_TRANSITION = 12000.0, 16000.0, 4000.0
+
+
+def probe_carriers(carriers, input_rate, iq, fmt, interpolation=1, decimation=None, seconds=None, nfft=16384, stream=None,
+                   device=0, **params):
+    """Identifies find_carriers' candidates from the IQ stream itself: one Ddc puts every candidate's center_hz at 12 kHz of 48 kHz
+    audio (decimation None: the ratio from rate_ratio), an Identifier on the same CUDA stream averages the squared spectra of the
+    first `seconds` (all of it when None), fed in 0.1 s writes, and identify() classifies each channel (params: its thresholds).
+
+    iq: interleaved host IQ as Ddc.write takes it, or (device pointer, n_iq). stream: a cudaStream_t as an int; None runs on a
+    new torch CUDA stream. -> new carrier dicts for channel_plan: mode the identified mode, center_hz moved by carrier_hz - 12 kHz,
+    plus fb_hz, ident_score_db (the best mode's score) and width_mode (find_carriers' width hint). A carrier whose identified
+    centre lies outside its candidate's [lo_hz, hi_hz] (a stronger neighbour's, say) is "unknown", and an unknown carrier keeps
+    the centre find_carriers measured."""
+    cands = list(carriers)
+    if not cands:
+        return []
+    if decimation is None:
+        interpolation, decimation = rate_ratio(input_rate)
+    out_rate = float(input_rate) * int(interpolation) / int(decimation)
+    if isinstance(iq, tuple):
+        dev_ptr, n_iq = int(iq[0]), int(iq[1])
+        if fmt not in Ddc.FORMATS:
+            raise ValueError("IQ format is 'cu8' or 'cs16'")
+        iq_bytes = 2 if Ddc.FORMATS[fmt] == IQ_CU8 else 4
+    else:
+        dev_ptr, (iq, _) = None, Ddc._iq(iq, fmt)
+        n_iq = iq.size // 2
+    if seconds is not None:
+        n_iq = min(n_iq, int(round(float(seconds) * float(input_rate))))
+    keep = None
+    if stream is None:
+        import torch
+        keep = torch.cuda.Stream(device=device)
+        stream = keep.cuda_stream
+    top = max(float(c.get("power", 0.0)) for c in cands)
+    gain = 0.2 * np.sqrt(2) / np.sqrt(top) if top > 0 else 1.0
+    ddc = Ddc(input_rate, decimation, [c["center_hz"] for c in cands], PROBE_AUDIO_HZ, PROBE_BANDWIDTH, PROBE_TRANSITION,
+              gain=gain, device=device, interpolation=interpolation)
+    ident = None
+    try:
+        ident = Identifier(out_rate, len(cands), nfft=nfft, device=device)
+        ddc.set_stream(stream); ident.set_stream(stream)
+        step = max(1, int(round(0.1 * float(input_rate))))
+        for a in range(0, n_iq, step):
+            m = min(step, n_iq - a)
+            if dev_ptr is None:
+                ddc.write(iq[2 * a:2 * (a + m)], fmt)
+            else:
+                ddc.write_device(dev_ptr + a * iq_bytes, m, fmt)
+            p, n, st = ddc.output()
+            if n:
+                ident.write_device(p, n, st)
+        sq, frames = ident.read()
+    finally:
+        if ident is not None:
+            ident.close()
+        ddc.close()
+        del keep
+    out = []
+    for c, row in zip(cands, sq):
+        r = identify(row, out_rate, frames, **params)
+        d = dict(c)
+        d["width_mode"] = c["mode"]
+        d["fb_hz"] = r["fb_hz"]
+        d["ident_score_db"] = max(r["score_db"].values())
+        center = c["center_hz"] + r["carrier_hz"] - PROBE_AUDIO_HZ
+        if r["mode"] != "unknown" and c["lo_hz"] <= center <= c["hi_hz"]:
+            d["mode"], d["center_hz"] = r["mode"], center
+        else:
+            d["mode"] = "unknown"
+        out.append(d)
+    return out

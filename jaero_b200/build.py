@@ -20,6 +20,7 @@ UNITS = [
     ("ddc.cu", []),
     ("resample.cu", []),
     ("scan.cu", []),
+    ("ident.cu", []),
     ("prefilter.cu", ["-fmad=false"]),
     ("fastfir.cu", ["-fmad=false"]),
     ("burst.cu", ["-fmad=false"]),

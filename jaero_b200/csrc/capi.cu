@@ -13,6 +13,7 @@
 #include "ddc.cuh"
 #include "scan.cuh"
 #include "resample.cuh"
+#include "ident.cuh"
 #include <cstring>
 #include <complex>
 #include <climits>
@@ -2842,3 +2843,216 @@ extern "C" int jaero_scan_find_carriers(const double *psd, int nfft, double inpu
     *n_found = found;
     return JAERO_OK;
 }
+
+// ------------------------------------------------------------------ mode identifier
+struct jaero_ident {
+    int device; cudaStream_t stream, own_stream;
+    std::vector<void *> allocs;
+    IdentPlan p;
+    long long n_in, frames, launches;                                 // samples and complete frames per channel since create / reset
+    int16_t *d_carry;                                                // [C][nfft] samples frames * hop .. n_in - 1 (fewer than nfft)
+    int16_t *d_in; size_t in_cap;                                    // host writes: the PCM staged on the device, [C][n]
+    int16_t *d_x; size_t x_cap;                                      // [C][carry + n] the samples the write's frames read
+    double2 *d_w0, *d_w1;                                            // [G][nfft] work matrices of one pass
+};
+
+static bool ident_nfft_ok(int nfft) { return nfft >= 1024 && nfft <= 16384 && (nfft & (nfft - 1)) == 0; }
+static bool ident_fs_ok(double fs) { return std::isfinite(fs) && fs >= 8000 && fs <= 192000 && fs == floor(fs); }
+static int ident_pass_frames(int nfft) { return (int)std::max<long long>(1, IDENT_PASS_ELEMS / nfft); }
+
+extern "C" {
+
+int jaero_ident_create(double Fs, int n_channels, int nfft, int device, jaero_ident **out)
+{
+    const char *fn = "jaero_ident_create";
+    if (!out || n_channels <= 0) { set_error(std::string(fn) + ": bad argument"); return JAERO_E_ARG; }
+    if (!ident_nfft_ok(nfft)) { set_error(std::string(fn) + ": nfft must be a power of two from 1024 to 16384"); return JAERO_E_ARG; }
+    if (!ident_fs_ok(Fs)) { set_error(std::string(fn) + ": Fs must be whole hertz from 8000 to 192000"); return JAERO_E_ARG; }
+    CreateGuard<jaero_ident> guard(jaero_ident_destroy);
+    { const int e = guard.begin(fn, device); if (e) return e; }
+    jaero_ident *d = guard.obj;
+    d->own_stream = d->stream;
+    IdentPlan &p = d->p;
+    p.nfft = nfft; p.hop = nfft / 2; p.n_channels = n_channels;
+    int lg = 0;
+    while ((1 << lg) < nfft) lg++;
+    p.n1 = 1 << (lg / 2); p.n2 = nfft / p.n1;
+    std::vector<double2> tw(nfft);
+    std::vector<double> win(nfft);
+    double wss = 0.0;
+    for (int k = 0; k < nfft; k++) {
+        const double a = 2 * M_PI * (double)k / nfft;
+        tw[k] = make_double2(cos(a), -sin(a));
+        win[k] = 0.5 - 0.5 * cos(a);
+        wss += win[k] * win[k];
+    }
+    p.inv_wss2 = 1.0 / (wss * wss);
+    const size_t work = (size_t)ident_pass_frames(nfft) * nfft;
+    double2 *dtw; double *dwin;
+    int rc = 0;
+    rc |= owned_alloc(d, &dtw, (size_t)nfft); rc |= owned_alloc(d, &dwin, (size_t)nfft);
+    rc |= owned_alloc(d, &p.sum, (size_t)n_channels * nfft);
+    rc |= owned_alloc(d, &d->d_carry, (size_t)n_channels * nfft);
+    rc |= owned_alloc(d, &d->d_w0, work); rc |= owned_alloc(d, &d->d_w1, work);
+    if (rc) return JAERO_E_CUDA;
+    p.tw = dtw; p.win = dwin;
+    JB_CUDA(cudaMemcpyAsync(dtw, tw.data(), nfft * sizeof(double2), cudaMemcpyHostToDevice, d->stream));
+    JB_CUDA(cudaMemcpyAsync(dwin, win.data(), nfft * sizeof(double), cudaMemcpyHostToDevice, d->stream));
+    JB_CUDA(cudaStreamSynchronize(d->stream));                       // the tables are in place, the host vectors may go
+    *out = guard.release();
+    return JAERO_OK;
+}
+void jaero_ident_destroy(jaero_ident *d)
+{
+    if (!d) return;
+    cudaSetDevice(d->device);
+    cudaStreamSynchronize(d->stream);
+    release(d, {d->d_in, d->d_x}, {}, d->own_stream);
+}
+int64_t jaero_ident_launch_count(const jaero_ident *d) { return d ? d->launches : 0; }
+
+int jaero_ident_write_device(jaero_ident *d, const int16_t *d_pcm, size_t n, size_t stride)
+{
+    if (!d || !d_pcm) { set_error("jaero_ident_write_device: null argument"); return JAERO_E_ARG; }
+    if ((uintptr_t)d_pcm & 1) { set_error("jaero_ident_write_device: PCM pointer not aligned to one sample"); return JAERO_E_ARG; }
+    if (stride < n) { set_error("jaero_ident_write_device: channel stride is smaller than n_samples"); return JAERO_E_ARG; }
+    if (n > ((size_t)1 << 34)) { set_error("jaero_ident_write_device: too many samples in one write"); return JAERO_E_ARG; }
+    if (n == 0) return JAERO_OK;
+    JB_CUDA(cudaSetDevice(d->device));
+    const IdentPlan &p = d->p;
+    const size_t C = (size_t)p.n_channels, B = sizeof(int16_t);
+    const long long N = p.nfft, hop = p.hop, total = d->n_in + (long long)n;
+    const long long x0 = d->frames * hop, carry = d->n_in - x0;      // d_x[c][j] = sample x0 + j of channel c
+    const long long f_end = total >= N ? (total - N) / hop + 1 : 0, F = f_end - d->frames;
+    if (F == 0) {                                                    // no frame completes: the samples join the carry
+        JB_CUDA(cudaMemcpy2DAsync(d->d_carry + carry, N * B, d_pcm, stride * B, n * B, C, cudaMemcpyDeviceToDevice, d->stream));
+        d->n_in = total;
+        return JAERO_OK;
+    }
+    const size_t pitch = (size_t)(carry + (long long)n);
+    // every buffer is in place before anything is queued: a failed write leaves the average unchanged
+    if (grow(&d->d_x, &d->x_cap, C * pitch, d->stream)) return JAERO_E_CUDA;
+    if (carry) JB_CUDA(cudaMemcpy2DAsync(d->d_x, pitch * B, d->d_carry, N * B, carry * B, C, cudaMemcpyDeviceToDevice, d->stream));
+    JB_CUDA(cudaMemcpy2DAsync(d->d_x + carry, pitch * B, d_pcm, stride * B, n * B, C, cudaMemcpyDeviceToDevice, d->stream));
+    if (ident_frames(p, d->d_x, pitch, x0, d->frames, F, ident_pass_frames(p.nfft), d->d_w0, d->d_w1, d->stream, &d->launches))
+        return JAERO_E_CUDA;
+    const long long x1 = f_end * hop;                                // the first sample an incomplete frame needs
+    if (total > x1)
+        JB_CUDA(cudaMemcpy2DAsync(d->d_carry, N * B, d->d_x + (x1 - x0), pitch * B, (total - x1) * B, C, cudaMemcpyDeviceToDevice, d->stream));
+    d->n_in = total; d->frames = f_end;
+    return JAERO_OK;
+}
+int jaero_ident_write(jaero_ident *d, const int16_t *pcm, size_t n, size_t stride)
+{
+    if (!d || !pcm) { set_error("jaero_ident_write: null argument"); return JAERO_E_ARG; }
+    if (stride < n) { set_error("jaero_ident_write: channel stride is smaller than n_samples"); return JAERO_E_ARG; }
+    if (n > ((size_t)1 << 34)) { set_error("jaero_ident_write: too many samples in one write"); return JAERO_E_ARG; }
+    JB_CUDA(cudaSetDevice(d->device));
+    const size_t C = (size_t)d->p.n_channels;
+    if (grow(&d->d_in, &d->in_cap, std::max<size_t>(C * n, 1), d->stream)) return JAERO_E_CUDA;
+    if (n) {
+        JB_CUDA(cudaMemcpy2DAsync(d->d_in, n * sizeof(int16_t), pcm, stride * sizeof(int16_t), n * sizeof(int16_t), C, cudaMemcpyHostToDevice,
+                                  d->stream));
+        JB_CUDA(cudaStreamSynchronize(d->stream));                   // the caller may reuse its pageable buffer on return
+    }
+    return jaero_ident_write_device(d, d->d_in, n, n);
+}
+int jaero_ident_set_stream(jaero_ident *d, void *cuda_stream)
+{
+    if (!d) { set_error("null handle"); return JAERO_E_ARG; }
+    JB_CUDA(cudaSetDevice(d->device));
+    JB_CUDA(cudaStreamSynchronize(d->stream));
+    d->stream = cuda_stream ? (cudaStream_t)cuda_stream : d->own_stream;
+    return JAERO_OK;
+}
+int jaero_ident_reset(jaero_ident *d)
+{
+    if (!d) { set_error("null handle"); return JAERO_E_ARG; }
+    JB_CUDA(cudaSetDevice(d->device));
+    JB_CUDA(cudaMemsetAsync(d->p.sum, 0, (size_t)d->p.n_channels * d->p.nfft * sizeof(double), d->stream));
+    d->n_in = 0; d->frames = 0;
+    return JAERO_OK;
+}
+int jaero_ident_read(jaero_ident *d, double *sq_mean, int64_t *frames)
+{
+    if (!d) { set_error("null handle"); return JAERO_E_ARG; }
+    JB_CUDA(cudaSetDevice(d->device));
+    const size_t total = (size_t)d->p.n_channels * d->p.nfft;
+    if (sq_mean) JB_CUDA(cudaMemcpyAsync(sq_mean, d->p.sum, total * sizeof(double), cudaMemcpyDeviceToHost, d->stream));
+    JB_CUDA(cudaStreamSynchronize(d->stream));
+    if (sq_mean && d->frames > 0)
+        for (size_t i = 0; i < total; i++) sq_mean[i] /= (double)d->frames;
+    if (frames) *frames = d->frames;
+    return JAERO_OK;
+}
+
+// Host only. The line pair of each JAERO rate in the squared spectrum (contract in include/jaero_b200.h).
+int jaero_ident_classify(const double *sq_mean, int nfft, double Fs, const jaero_ident_params *params, jaero_ident_result *out)
+{
+    const char *fn = "jaero_ident_classify";
+    if (!sq_mean || !out) { set_error(std::string(fn) + ": null argument"); return JAERO_E_ARG; }
+    if (!ident_nfft_ok(nfft)) { set_error(std::string(fn) + ": nfft must be a power of two from 1024 to 16384"); return JAERO_E_ARG; }
+    if (!ident_fs_ok(Fs)) { set_error(std::string(fn) + ": Fs must be whole hertz from 8000 to 192000"); return JAERO_E_ARG; }
+    const jaero_ident_params P = params ? *params : jaero_ident_params{5.0, 400.0, 0.5};
+    if (!std::isfinite(P.threshold_db) || !(P.floor_window_hz > 0) || !std::isfinite(P.floor_window_hz) ||
+        !(P.floor_quantile >= 0 && P.floor_quantile <= 1)) { set_error(std::string(fn) + ": parameter out of range"); return JAERO_E_ARG; }
+    const int n = nfft;
+    for (int i = 0; i < n; i++)
+        if (!(sq_mean[i] >= 0) || !std::isfinite(sq_mean[i])) { set_error(std::string(fn) + ": spectrum values must be finite and >= 0"); return JAERO_E_ARG; }
+    const double bin_hz = Fs / n;
+    const double x = std::min(P.floor_window_hz / bin_hz, (double)n);
+    const int W = std::min(std::max(2 * (int)std::floor(x / 2) + 1, 3), n);
+    std::vector<double> fl(n), Q(n);
+    scan_floor(sq_mean, n, W, P.floor_quantile, fl.data());
+    for (int i = 0; i < n; i++) Q[i] = fl[i] > 0 ? sq_mean[i] / fl[i] : 0.0;
+    static const double fbs[4] = {600.0, 1200.0, 8400.0, 10500.0};
+    static const int modes[4] = {JAERO_MODE_MSK600, JAERO_MODE_MSK1200, JAERO_MODE_OQPSK8400, JAERO_MODE_OQPSK10500};
+    double score[4];
+    long long li[4], lj[4];                                          // lower line's bin, upper line's unwrapped bin
+    for (int m = 0; m < 4; m++) {
+        const long long D = (long long)std::llround(fbs[m] * n / Fs);
+        score[m] = -1; li[m] = lj[m] = 0;
+        for (int i = 0; i < n; i++) {
+            long long jmax = 0; double qmax = -1;
+            for (int e = -1; e <= 1; e++) {
+                const long long j = i + D + e;
+                const double q = Q[(size_t)(((j % n) + n) % n)];
+                if (q > qmax) { qmax = q; jmax = j; }
+            }
+            const double s = std::min(Q[i], qmax);
+            if (s > score[m]) { score[m] = s; li[m] = i; lj[m] = jmax; }
+        }
+    }
+    jaero_ident_result r;
+    std::memset(&r, 0, sizeof r);
+    int best = 0;
+    for (int m = 0; m < 4; m++) {
+        r.score_db[m] = score[m] > 0 ? 10 * log10(score[m]) : -HUGE_VAL;
+        if (score[m] > score[best]) best = m;
+    }
+    double other = -HUGE_VAL;
+    for (int m = 0; m < 4; m++)
+        if (m != best) other = std::max(other, r.score_db[m]);
+    r.margin_db = r.score_db[best] - other;
+    auto refine = [&](long long k) {                                 // log-parabolic offset of the line at bin k mod n
+        const int c = (int)(((k % n) + n) % n);
+        const double y0 = sq_mean[(c + n - 1) % n], y1 = sq_mean[c], y2 = sq_mean[(c + 1) % n];
+        if (!(y0 > 0 && y1 > 0 && y2 > 0)) return 0.0;
+        const double l0 = log(y0), l1 = log(y1), l2 = log(y2), den = l0 - 2 * l1 + l2;
+        if (den == 0) return 0.0;
+        return std::min(0.5, std::max(-0.5, (l0 - l2) / (2 * den)));
+    };
+    const double di = refine(li[best]), dj = refine(lj[best]);
+    const double lo = (double)li[best] + di, hi = (double)lj[best] + dj;
+    r.line_hz[0] = (lo - n / 2) * bin_hz;
+    r.line_hz[1] = ((double)(((lj[best] % n) + n) % n) + dj - n / 2) * bin_hz;
+    r.fb_hz = (hi - lo) * bin_hz;
+    const double mid = (0.5 * (lo + hi) - n / 2) * bin_hz;
+    r.carrier_hz = fmod(fmod(mid, Fs) + Fs, Fs) / 2;
+    r.frames = 0;
+    r.mode = r.score_db[best] >= P.threshold_db ? modes[best] : JAERO_MODE_UNKNOWN;
+    *out = r;
+    return JAERO_OK;
+}
+
+} // extern "C"
