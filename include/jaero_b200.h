@@ -228,7 +228,10 @@ typedef struct jaero_pchannel jaero_pchannel;
 int jaero_pchannel_create(int n_channels, double fb, int device_ordinal, jaero_pchannel **out);
 void jaero_pchannel_destroy(jaero_pchannel *p);
 /* Consume everything the batch's demodulators emitted since the last call (device-resident, no host hop),
- * run framing + de-interleave + Viterbi + descramble + CRC, and write each channel's DCD back into the batch. */
+ * run framing + de-interleave + Viterbi + descramble + CRC, and write each channel's DCD back into the batch.
+ * Known deviation (DESIGN.md §8): a frame's CRC-driven DCD countdown updates land at the end of the call that completed it,
+ * after any UW sync later in that call, and a DCD they raise does not stop the 10.5 kbps UW search within that call. The DCD
+ * written back to the demodulators follows the same rule. */
 int jaero_pchannel_process_batch(jaero_pchannel *p, jaero_batch *b);
 /* Same for soft bits supplied by the host: soft[ch*cap + k], counts[ch] (drop-in for processDemodulatedSoftBits). */
 int jaero_pchannel_process_softbits(jaero_pchannel *p, const int16_t *soft, size_t cap_per_channel, const int32_t *counts);

@@ -1973,7 +1973,7 @@ int jaero_cchannel_create(int n_channels, int device, jaero_cchannel **out)
     cp.n_channels = n_channels; cp.dl2_len = 2714 - 6 + 1;                     // dl2.setLength(2714-6) (aerol.cpp:1037)
     const size_t C = n_channels;
     int rc = 0;
-    rc |= owned_alloc(c, &cp.state, C); rc |= owned_alloc(c, &cp.coded, C * CC_QUEUE * CC_CODED_PITCH); rc |= owned_alloc(c, &cp.decoded, C * CC_QUEUE * CC_DEC);
+    rc |= owned_alloc(c, &cp.state, C); rc |= owned_alloc(c, &cp.coded, C * CC_SLOTS * CC_CODED_PITCH); rc |= owned_alloc(c, &cp.decoded, C * CC_QUEUE * CC_DEC);
     rc |= owned_alloc(c, &cp.ready, C); rc |= owned_alloc(c, &cp.dl2, C * cp.dl2_len); rc |= owned_alloc(c, &cp.out, C * CC_OUT * CC_RECORD);
     rc |= owned_alloc(c, &c->vit_overlap, C * 64); rc |= owned_alloc(c, &c->vit_overlap_len, C); rc |= owned_alloc(c, &c->vit_renorm, C); rc |= owned_alloc(c, &c->vit_valid, C);
     if (rc) return JAERO_E_CUDA;

@@ -42,7 +42,7 @@ cchan_frame_kernel(CChanParams cp, const int16_t *__restrict__ soft, const int *
     CChanState s = cp.state[ch];
     const int n = soft_count[ch];
     const int16_t *bits = soft + (size_t)ch * soft_stride;
-    uint8_t *coded = cp.coded + (size_t)ch * CC_QUEUE * CC_CODED_PITCH;
+    uint8_t *coded = cp.coded + (size_t)ch * CC_SLOTS * CC_CODED_PITCH;
     if (s.carry_slot > 0) {
         // the frame that was being filled when the previous call ended sits in slot `carry_slot`: it continues in slot 0
         const int4 *src = reinterpret_cast<const int4 *>(coded + (size_t)s.carry_slot * CC_CODED_PITCH);
@@ -69,15 +69,16 @@ cchan_frame_kernel(CChanParams cp, const int16_t *__restrict__ soft, const int *
                 const int c = s.cntr, b = c >> 8, idx = c & 255, r = idx >> 2, j = idx & 3;
                 const int k = j * 64 + ((r * 19) & 63);                                       // 19 = 27^-1 mod 64
                 const int p = 256 * b + k;
-                if (p < CC_FRAME_BITS - 1 && s.frames_ready < CC_QUEUE) coded[(size_t)s.frames_ready * CC_CODED_PITCH + p + p / 3] = (uint8_t)soft_bit;
+                // row frames_ready: after a full queue the next frame still has a row, so it can finish in the next call
+                if (p < CC_FRAME_BITS - 1) coded[(size_t)s.frames_ready * CC_CODED_PITCH + p + p / 3] = (uint8_t)soft_bit;
             }
             if (s.cntr == CC_FRAME_BITS - 1) {                                                 // frame complete
-                if (s.frames_ready < CC_QUEUE) s.frames_ready++; else s.overflow = 1;
+                if (s.frames_ready < CC_QUEUE) s.frames_ready++; else s.overflow = 1;    // a fifth frame in one call is lost (reported)
             }
         }
     }
     lost.finish(s);
-    s.carry_slot = (s.frames_ready > 0 && s.frames_ready < CC_QUEUE) ? s.frames_ready : 0;
+    s.carry_slot = s.frames_ready;
     cp.state[ch] = s;
     cp.ready[ch] = s.frames_ready;
 }
@@ -143,8 +144,8 @@ __global__ void cchan_init_kernel(CChanParams cp)
     memset(&s, 0, sizeof s);
     s.cntr = CNTR_IDLE;                                        // AeroL ctor (aerol.cpp:907,927); index = 0 (:957)
     cp.state[ch] = s;
-    uint8_t *coded = cp.coded + (size_t)ch * CC_QUEUE * CC_CODED_PITCH;
-    for (int q = 0; q < CC_QUEUE; q++) for (int k = 0; k < CC_CODED_PITCH; k++) coded[(size_t)q * CC_CODED_PITCH + k] = 128;   // erasure slots
+    uint8_t *coded = cp.coded + (size_t)ch * CC_SLOTS * CC_CODED_PITCH;
+    for (int q = 0; q < CC_SLOTS; q++) for (int k = 0; k < CC_CODED_PITCH; k++) coded[(size_t)q * CC_CODED_PITCH + k] = 128;   // erasure slots
 }
 
 int cchan_process(const CChanParams &cp, const int16_t *d_soft, const int *d_soft_count, size_t soft_stride, int *demod_dcd,
@@ -157,7 +158,7 @@ int cchan_process(const CChanParams &cp, const int16_t *d_soft, const int *d_sof
     (*launches)++;
     for (int q = 0; q < CC_QUEUE; q++) {
         if (viterbi_launch(cp.coded + (size_t)q * CC_CODED_PITCH, CC_CODED, 0, 0, 24, vit_overlap, vit_overlap_len, vit_renorm,
-                           cp.decoded + (size_t)q * CC_DEC, vit_valid, cp.n_channels, st, (size_t)CC_QUEUE * CC_CODED_PITCH, (size_t)CC_QUEUE * CC_DEC,
+                           cp.decoded + (size_t)q * CC_DEC, vit_valid, cp.n_channels, st, (size_t)CC_SLOTS * CC_CODED_PITCH, (size_t)CC_QUEUE * CC_DEC,
                            cp.ready, q)) return -1;
         (*launches)++;
     }

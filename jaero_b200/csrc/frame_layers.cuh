@@ -54,6 +54,7 @@ static const int CC_CODED_PITCH = 5472;    // row pitch (16-byte multiple)
 static const int CC_DEC = 2730;            // decoded bits per frame before resize(2714)
 static const int CC_KEEP = 2714;
 static const int CC_QUEUE = 4;             // frames that may complete per channel in one call
+static const int CC_SLOTS = CC_QUEUE + 1;  // code-order rows per channel: the queue and the frame still being filled after it
 static const int CC_OUT = 8;               // decoded frames held per channel until read
 static const int CC_RECORD = 352;          // 3 x (12 SU bytes + crc flag + 3 pad) + 300 voice bytes + 4 (frame number)
 
@@ -67,7 +68,7 @@ struct CChanState {
 struct CChanParams {
     int n_channels, dl2_len;
     CChanState *state;
-    uint8_t *coded;         // [ch][CC_QUEUE][CC_CODED_PITCH] code-order soft values (erasures = 128 pre-filled)
+    uint8_t *coded;         // [ch][CC_SLOTS][CC_CODED_PITCH] code-order soft values (erasures = 128 pre-filled)
     uint8_t *decoded;       // [ch][CC_QUEUE][CC_DEC]
     int *ready;             // [ch]
     uint8_t *dl2;           // [ch][dl2_len]
@@ -114,7 +115,7 @@ int frame_set_scrambler();                 // AeroLScrambler::pre_state into the
 template <class State> int frame_tick(State *state, int n_channels, int *demod_dcd, cudaStream_t st);
 // AeroL::LostSignal on one channel (>= 0) or all (-1); P- and C-channel
 template <class State> int frame_lost(State *state, int n_channels, int channel, int *demod_dcd, cudaStream_t st);
-// the decoded-record queue has been read out; C-channel and R/T
+// the decoded-record queue has been read out: its count and overflow flag start again; C-channel and R/T
 template <class State> int frame_out_reset(State *state, int n_channels, cudaStream_t st);
 
 // a kernel with one thread per channel

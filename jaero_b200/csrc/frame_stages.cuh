@@ -140,10 +140,12 @@ template <class State> __global__ void frame_lost_kernel(State *state, int n_cha
     if (demod_dcd) demod_dcd[ch] = 0;
 }
 
+// The read has copied out the state with its overflow flag, which reported every record lost since the previous read: both
+// start again, so one overflow fails one read, not every later one.
 template <class State> __global__ void frame_out_reset_kernel(State *state, int n_channels)
 {
     const int ch = blockIdx.x * blockDim.x + threadIdx.x;
-    if (ch < n_channels) state[ch].out_count = 0;
+    if (ch < n_channels) { state[ch].out_count = 0; state[ch].overflow = 0; }
 }
 
 // The C API launches the kernels above through these: a template kernel is launched only in the unit that defines it, and

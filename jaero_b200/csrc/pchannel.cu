@@ -10,9 +10,12 @@
 //   2. viterbi (K5)         one launch per queue slot, de-interleave fused (viterbi.cu)
 //   3. pchan_su_kernel      DelayLine dl2 (aerol.h:451-481) -> AeroLScrambler (aerol.h:397-437) ->
 //                           LSB-first byte packing (:1568-1580) -> per-SU CRC (aerol.h:334-362) -> DCD countdown
-// Integer/byte work throughout: bit-exact against the oracle. Known deviation, stated in DESIGN.md: CRC-driven
+// Integer/byte work throughout: bit-exact against the oracle. Known deviation, stated in DESIGN.md §8: CRC-driven
 // updates of datacdcountdown (aerol.cpp:1601-1608) are applied after stage 3, i.e. at the end of the call that
-// completed the frame, not in the middle of the bit loop.
+// completed the frame, not in the middle of the bit loop. Two effects within one call: a UW sync after the frame's end
+// (which sets the countdown to 12) comes before the frame's updates instead of after them, so the countdown and the DCD
+// that later ticks leave can differ; and a frame whose CRCs raise DCD does not stop the 10.5 kbps detectors searching the
+// rest of the call, so an exact UW copy in the next frame's data region syncs here and not in the reference.
 #include <cstdint>
 #include "viterbi.cuh"
 #include "frame_stages.cuh"

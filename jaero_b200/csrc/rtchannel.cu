@@ -69,7 +69,8 @@ rt_frame_kernel(RtParams rp, const int16_t *__restrict__ soft, const int *__rest
                 // rtchanneldeleavefecscram.resetblockptr(): a new packet slot
                 slots[cur].fill = fill; slots[cur].closed = 1;
                 if (s.n_open < RT_SLOTS) { cur++; if (cur >= RT_SLOTS) cur = 0; s.n_open++; }
-                else s.overflow = 1;                                         // no slot left: the oldest pending packet of this call is lost (reported)
+                else s.overflow = 1;                                         // no slot left: the slot just closed is reused, so the packet that was
+                                                                             // being filled when this unique word arrived is lost (reported)
                 RtSlot ns; ns.fill = 0; ns.next_trial = rp.oqpsk ? 64 * 2 : 64 * 5; ns.done = 0; ns.closed = 0; ns.targetSUSize = 0; ns.targetBlocks = 0; ns.start_bit = s.bits_seen;
                 slots[cur] = ns;
                 fill = 0;

@@ -48,7 +48,7 @@ def lib():
         L.jor_conv_decode_soft.argtypes = [vp, i, vp]; L.jor_conv_encode.argtypes = [vp, i, vp]
         L.jor_pchan_new.restype = vp; L.jor_pchan_new.argtypes = [i]
         L.jor_pchan_process.argtypes = [vp, vp, i]; L.jor_pchan_update_dcd.argtypes = [vp]
-        L.jor_pchan_dcd.argtypes = [vp]
+        L.jor_pchan_dcd.argtypes = [vp]; L.jor_pchan_syncs.restype = l; L.jor_pchan_syncs.argtypes = [vp]
         L.jor_pchan_lost_signal.argtypes = [vp]; L.jor_wire_pchan.argtypes = [vp, vp]
         L.jor_pchan_su_count.restype = l; L.jor_pchan_su_count.argtypes = [vp]
         L.jor_pchan_su_take.restype = l; L.jor_pchan_su_take.argtypes = [vp, vp, vp, vp, l]
@@ -201,6 +201,11 @@ class OraclePChannel:
     def dcd(self):
         return bool(lib().jor_pchan_dcd(self.h))
 
+    @property
+    def syncs(self):
+        """unique-word syncs so far"""
+        return int(lib().jor_pchan_syncs(self.h))
+
     def take_sus(self):
         n = lib().jor_pchan_su_count(self.h)
         b = np.zeros((n, 12), dtype=np.uint8); ok = np.zeros(n, dtype=np.int32); fr = np.zeros(n, dtype=np.int64)
@@ -258,7 +263,7 @@ class OracleCChannel:
         L = lib()
         L.jor_cchan_new.restype = ctypes.c_void_p
         L.jor_cchan_process.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int]
-        L.jor_cchan_update_dcd.argtypes = [ctypes.c_void_p]
+        L.jor_cchan_update_dcd.argtypes = [ctypes.c_void_p]; L.jor_cchan_lost_signal.argtypes = [ctypes.c_void_p]
         L.jor_cchan_dcd.argtypes = [ctypes.c_void_p]
         L.jor_cchan_frame_count.restype = ctypes.c_long; L.jor_cchan_frame_count.argtypes = [ctypes.c_void_p]
         L.jor_cchan_take.restype = ctypes.c_long; L.jor_cchan_take.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_long]
@@ -271,6 +276,10 @@ class OracleCChannel:
 
     def update_dcd(self):
         lib().jor_cchan_update_dcd(self.h)
+
+    def lost_signal(self):
+        """AeroL::LostSignal (aerol.h:925-931)"""
+        lib().jor_cchan_lost_signal(self.h)
 
     @property
     def dcd(self):

@@ -82,7 +82,7 @@ PChannelOracle::PChannelOracle(int fb) : codec(24)
     cntr = 1000000000; blockcnt = -1;
     frameinfo = lastframeinfo = 0; formatid = supfrmaker = framecounter1 = framecounter2 = 0;
     datacdcountdown = 0; datacd = false;
-    nframes = 0; bits_seen = 0;
+    nframes = 0; bits_seen = 0; n_syncs = 0;
 }
 
 // PreambleDetectorPhaseInvariant::Update with tollerence 0 (aerol.cpp:781-804, non-burst :1003-1005)
@@ -187,7 +187,7 @@ void PChannelOracle::process(const short *bits, int n)
         }
         if (gotsync) {                                          // :1990-2011
             cntr = -1; datacd = true; datacdcountdown = 12; dcd_events.push_back((bits_seen << 1) | 1);
-            scr_pos = 0;
+            scr_pos = 0; n_syncs++;
         }
         if (cntr + 1 == TotalNumberOfBits) { scr_pos = 0; cntr = -1; }   // :2013-2016
     }
@@ -531,6 +531,7 @@ void CChannelOracle::updateDCD()
     else { if (datacdcountdown < 0) datacdcountdown = 0; }
     if (datacd && !datacdcountdown) datacd = false;
 }
+void CChannelOracle::lostSignal() { cntr = 1000000000; datacdcountdown = 0; datacd = false; }
 
 // ====================================================================================== pinning hooks
 // The pieces of this restatement one by one, for tests/test_fec_pinning.py, which holds them against the reference's own

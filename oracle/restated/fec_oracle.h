@@ -47,7 +47,7 @@ struct PChannelOracle
     // outputs
     std::vector<SignalUnit> sus;
     std::vector<long> dcd_events;                  // (bit index<<1)|dcd at every DataCarrierDetect emit
-    long bits_seen;
+    long bits_seen, n_syncs;                       // n_syncs: unique-word syncs so far
     explicit PChannelOracle(int fb);
     void process(const short *soft, int n);        // AeroL::processDemodulatedSoftBits -> Decode(bits,true)
     void updateDCD();                              // AeroL::updateDCD (aerol.cpp:1109-1122), 1 s tick
@@ -70,6 +70,7 @@ struct CChannelOracle
     CChannelOracle();
     void process(const short *soft, int n);
     void updateDCD();
+    void lostSignal();                             // AeroL::LostSignal (aerol.h:925-931): the members DecodeC uses
 };
 
 // ---- burst (R/T channel) branch of AeroL::Decode (JAERO/aerol.cpp:1124-1350, :1985-2031) with

@@ -135,6 +135,7 @@ void jor_wire_pchan(void *hv, void *pv)
 void jor_pchan_process(void *p, const short *soft, int n) { ((PChannelOracle *)p)->process(soft, n); }
 void jor_pchan_update_dcd(void *p) { ((PChannelOracle *)p)->updateDCD(); }
 int jor_pchan_dcd(void *p) { return ((PChannelOracle *)p)->datacd ? 1 : 0; }
+long jor_pchan_syncs(void *p) { return ((PChannelOracle *)p)->n_syncs; }
 long jor_pchan_su_count(void *p) { return (long)((PChannelOracle *)p)->sus.size(); }
 long jor_pchan_su_take(void *p, uint8_t *bytes12, int *crc_ok, long *frame, long cap)
 {
@@ -147,6 +148,7 @@ void jor_pchan_free(void *p) { delete (PChannelOracle *)p; }
 void *jor_cchan_new() { return new CChannelOracle(); }
 void jor_cchan_process(void *p, const short *soft, int n) { ((CChannelOracle *)p)->process(soft, n); }
 void jor_cchan_update_dcd(void *p) { ((CChannelOracle *)p)->updateDCD(); }
+void jor_cchan_lost_signal(void *p) { ((CChannelOracle *)p)->lostSignal(); }
 int jor_cchan_dcd(void *p) { return ((CChannelOracle *)p)->datacd ? 1 : 0; }
 long jor_cchan_frame_count(void *p) { return (long)((CChannelOracle *)p)->frames.size(); }
 // frames: su [n][3][12], crc_ok [n][3], voice [n][300]
