@@ -1020,9 +1020,6 @@ int jaero_batch_write_device(jaero_batch *b, const int16_t *d_pcm, size_t n, siz
                          [&](int i0, int i1, int fill0) { return fir_exchange_up_launch(b->pre, b->fir, i0, i1, fill0, b->stream); }))
             return JAERO_E_CUDA;
     }
-    peak_kernel<<<(p.n_channels + 3) / 4, 128, 0, b->stream>>>(p, d_pcm, stride, (int)n);
-    JB_CUDA(cudaGetLastError());
-    b->launches++;
     const int N = p.bbnfft, trig_every = p.cpu_reduce ? N : N / 4;
     SegmentArgs a;
     memset(&a, 0, sizeof a);
@@ -1079,6 +1076,11 @@ int jaero_batch_write_device(jaero_batch *b, const int16_t *d_pcm, size_t n, siz
     b->samples += ((int)n - seg_start);
     while (b->next_slice < b->n_slices) { JB_CUDA(cudaStreamWaitEvent(b->stream, b->ev_slice[b->next_slice], 0)); b->next_slice++; }
     b->n_slices = 0; b->next_slice = 0;
+    // PeakVolume reads the whole call: only here, after the wait for the last copy slice, is all of it staged (the segments
+    // above wait only for the slices they read)
+    peak_kernel<<<(p.n_channels + 3) / 4, 128, 0, b->stream>>>(p, d_pcm, stride, (int)n);
+    JB_CUDA(cudaGetLastError());
+    b->launches++;
     b->bb_pos = bb; b->coarse_counter = cc;
     if (b->pre_on) {                                               // :608 mixer_fir_pre.SetFreq(mixer2_freq_sum/i)
         if (pre_finish_launch(b->pre, p.m2_freq_sum, (int)n, p.Fs, b->stream)) return JAERO_E_CUDA;

@@ -34,6 +34,9 @@ def lib():
         L.jref_ebno_log_take.restype = l; L.jref_ebno_log_take.argtypes = [vp, vp, l]
         L.jref_write.argtypes = [vp, vp, l]
         L.jref_set_dcd.argtypes = [vp, i]
+        if hasattr(L, "jref_set_center_freq"):          # absent from a reference build made before it existed
+            L.jref_set_center_freq.argtypes = [vp, d]
+            L.jref_set_afc.argtypes = [vp, i]; L.jref_set_sql.argtypes = [vp, i]; L.jref_set_cpu_reduce.argtypes = [vp, i]
         L.jref_soft_count.restype = l; L.jref_soft_count.argtypes = [vp]
         L.jref_soft_take.restype = l; L.jref_soft_take.argtypes = [vp, vp, l]
         L.jref_emit_count.restype = l; L.jref_emit_count.argtypes = [vp]
@@ -127,6 +130,19 @@ class RefDemod:
     def set_dcd(self, dcd):
         lib().jref_set_dcd(self.h, int(dcd))
 
+    def set_center_freq(self, hz):
+        """the reference's own CenterFreqChangedSlot / setAFC / setSQL / setCPUReduce (continuous kinds)"""
+        lib().jref_set_center_freq(self.h, float(hz))
+
+    def set_afc(self, state):
+        lib().jref_set_afc(self.h, int(bool(state)))
+
+    def set_sql(self, state):
+        lib().jref_set_sql(self.h, int(bool(state)))
+
+    def set_cpu_reduce(self, state):
+        lib().jref_set_cpu_reduce(self.h, int(bool(state)))
+
     def take_soft(self):
         n = lib().jref_soft_count(self.h)
         out = np.zeros(n, dtype=np.int16)
@@ -179,15 +195,17 @@ class RefCodec:
 
 
 def run_demod_job(args):
-    """Process-pool worker: (kind, kwargs, pcm, chunk, dcd_schedule) -> (soft, state, cfe_log).
-    dcd_schedule: list of (sample_index, dcd) applied at chunk boundaries (index must be a multiple of chunk)."""
-    kind, kw, pcm, chunk, dcd_schedule = args
+    """Process-pool worker: (kind, kwargs, pcm, chunk, dcd_schedule[, events]) -> (soft, state, cfe_log).
+    dcd_schedule: list of (sample_index, dcd) applied at chunk boundaries (index must be a multiple of chunk).
+    events: control calls at sample indices, as restated.write_plan takes them; the writes are cut at each of them."""
+    from oracle.restated import apply_calls, write_plan
+    kind, kw, pcm, chunk, dcd_schedule = args[:5]
+    events = list(args[5]) if len(args) > 5 and args[5] else []
+    events += [(int(a), [("set_dcd", int(v))]) for a, v in (dcd_schedule or [])]
     d = RefDemod(kind, **kw)
-    sched = dict(dcd_schedule or [])
-    for a in range(0, len(pcm), chunk):
-        if a in sched:
-            d.set_dcd(sched[a])
-        d.write(pcm[a:a + chunk])
+    for a, n, calls in write_plan(len(pcm), chunk, events):
+        apply_calls(d, calls)
+        d.write(pcm[a:a + n])
     out = (d.take_soft(), d.state(), d.take_cfe_log())
     d.close()
     return out

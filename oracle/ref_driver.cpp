@@ -174,6 +174,15 @@ void jref_set_dcd(void *hv, int dcd)
     else if (h->kind == 1) h->msk->DCDstatSlot(dcd != 0);
     else if (h->kind == 2) h->bmsk->DCDstatSlot(dcd != 0);
 }
+// the run-time controls, through the reference's own slots (oqpskdemodulator.cpp:149-167,291-310, mskdemodulator.cpp:105-122,265-282)
+void jref_set_center_freq(void *hv, double hz)
+{ RefHandle *h = (RefHandle *)hv; if (h->kind == 0) h->oq->CenterFreqChangedSlot(hz); else if (h->kind == 1) h->msk->CenterFreqChangedSlot(hz); }
+void jref_set_afc(void *hv, int v)
+{ RefHandle *h = (RefHandle *)hv; if (h->kind == 0) h->oq->setAFC(v != 0); else if (h->kind == 1) h->msk->setAFC(v != 0); }
+void jref_set_sql(void *hv, int v)
+{ RefHandle *h = (RefHandle *)hv; if (h->kind == 0) h->oq->setSQL(v != 0); else if (h->kind == 1) h->msk->setSQL(v != 0); }
+void jref_set_cpu_reduce(void *hv, int v)
+{ RefHandle *h = (RefHandle *)hv; if (h->kind == 0) h->oq->setCPUReduce(v != 0); else if (h->kind == 1) h->msk->setCPUReduce(v != 0); }
 long jref_ebno_log_take(void *hv, double *out, long cap)
 {
     RefHandle *h = (RefHandle *)hv;

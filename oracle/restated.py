@@ -31,6 +31,8 @@ def lib():
         L.jor_burst_oqpsk_new.restype = vp; L.jor_burst_oqpsk_new.argtypes = [d, d, d, d, d]
         L.jor_aux_take.restype = l; L.jor_aux_take.argtypes = [vp, i, vp, l]
         L.jor_write.argtypes = [vp, vp, l]; L.jor_set_dcd.argtypes = [vp, i]
+        L.jor_set_center_freq.argtypes = [vp, d]
+        L.jor_set_afc.argtypes = [vp, i]; L.jor_set_sql.argtypes = [vp, i]; L.jor_set_cpu_reduce.argtypes = [vp, i]
         L.jor_burst_set_sql.argtypes = [vp, i]
         L.jor_soft_count.restype = l; L.jor_soft_count.argtypes = [vp]
         L.jor_soft_take.restype = l; L.jor_soft_take.argtypes = [vp, vp, l]
@@ -81,6 +83,20 @@ class OracleDemod:
 
     def set_dcd(self, dcd):
         lib().jor_set_dcd(self.h, int(dcd))
+
+    def set_center_freq(self, hz):
+        """CenterFreqChangedSlot (continuous kinds)"""
+        lib().jor_set_center_freq(self.h, float(hz))
+
+    def set_afc(self, state):
+        """setAFC / setSQL / setCPUReduce (continuous kinds): plain flags, read by the following writes"""
+        lib().jor_set_afc(self.h, int(bool(state)))
+
+    def set_sql(self, state):
+        lib().jor_set_sql(self.h, int(bool(state)))
+
+    def set_cpu_reduce(self, state):
+        lib().jor_set_cpu_reduce(self.h, int(bool(state)))
 
     def take_soft(self):
         n = lib().jor_soft_count(self.h)
@@ -297,19 +313,47 @@ class OracleCChannel:
             lib().jor_cchan_free(self.h); self.h = None
 
 
+CONTROLS = ("set_center_freq", "set_afc", "set_sql", "set_cpu_reduce", "set_dcd")
+
+
+def write_plan(n, chunk, events=()):
+    """[(start, length, calls)]: n samples written in pieces of `chunk` samples (or of the successive lengths in `chunk` when
+    it is a sequence), each piece cut again at every event position. events: [(sample_index, [(name, *args), ...]), ...] with
+    names from CONTROLS; an event's calls are made before the write that starts at its sample index."""
+    ev = {}
+    for at, calls in events or ():
+        at = int(at)
+        assert 0 <= at < n, at
+        assert all(c[0] in CONTROLS for c in calls), calls
+        ev.setdefault(at, []).extend(tuple(c) for c in calls)
+    sizes = [chunk] * -(-n // chunk) if np.ndim(chunk) == 0 else list(chunk)
+    cuts, a = set(ev), 0
+    for m in sizes:
+        cuts.add(a); a += int(m)
+        if a >= n:
+            break
+    assert a >= n, "the write sizes cover %d of %d samples" % (a, n)
+    cuts = sorted(c for c in cuts if c < n) + [n]
+    return [(a, b - a, ev.get(a, [])) for a, b in zip(cuts[:-1], cuts[1:])]
+
+
+def apply_calls(demod, calls):
+    """make each (name, *args) call of an event on a demodulator (OracleDemod, RefDemod or DemodBatch)"""
+    for name, *args in calls:
+        getattr(demod, name)(*args)
+
+
 def run_demod_job(args):
-    """(kind, kw, pcm, chunk) -> (soft, state, aux0): one restated demodulator over one stream, written in pieces of `chunk`
-    samples, or of the successive lengths in `chunk` when it is a sequence. Module-level so that tests can farm channels out to a
-    multiprocessing pool."""
-    kind, kw, pcm, chunk = args
+    """(kind, kw, pcm, chunk[, events]) -> (soft, state, aux): one restated demodulator over one stream, written in pieces of
+    `chunk` samples, or of the successive lengths in `chunk` when it is a sequence, with the control calls of `events` made at
+    their sample indices (write_plan). aux: the EbNo of each burst (burst kinds) or the emitted coarse estimates. Module-level so that tests can farm channels out to a multiprocessing pool."""
+    kind, kw, pcm, chunk = args[:4]
+    events = args[4] if len(args) > 4 else ()
     d = OracleDemod(kind, **kw)
-    if np.ndim(chunk) == 0:
-        chunk = [chunk] * -(-len(pcm) // chunk)
-    a = 0
-    for n in chunk:
-        d.write(pcm[a:a + n]); a += n
-    assert a >= len(pcm)
+    for a, n, calls in write_plan(len(pcm), chunk, events):
+        apply_calls(d, calls)
+        d.write(pcm[a:a + n])
     soft, st = d.take_soft(), d.state()
-    aux = d.take_aux(0) if kind.startswith("burst") else np.zeros(0)
+    aux = d.take_aux(0) if kind.startswith("burst") else d.take_cfe_log()
     d.close()
     return soft, st, aux

@@ -278,6 +278,19 @@ void OqpskDemodOracle::FreqOffsetEstimateSlot(double est)
     if (on_sigstat) on_sigstat(hook_ctx, !(mse > s.signalthreshold));
 }
 
+void OqpskDemodOracle::CenterFreqChangedSlot(double freq_center)
+{
+    if (s.fb != 8400) {                                                                         // :293-297
+        if (freq_center < (0.5 * s.fb)) freq_center = 0.5 * s.fb;
+        if (freq_center > (s.Fs / 2.0 - 0.5 * s.fb)) freq_center = s.Fs / 2.0 - 0.5 * s.fb;
+    }
+    mixer_center.SetFreq(freq_center, (int)s.Fs);                                               // :298
+    if (s.afc) mixer2.SetFreq(mixer_center.GetFreqHz());                                        // :299
+    if ((mixer2.GetFreqHz() - mixer_center.GetFreqHz()) > (s.lockingbw / 2.0)) mixer2.SetFreq(mixer_center.GetFreqHz() + (s.lockingbw / 2.0));    // :300-303
+    if ((mixer2.GetFreqHz() - mixer_center.GetFreqHz()) < (-s.lockingbw / 2.0)) mixer2.SetFreq(mixer_center.GetFreqHz() - (s.lockingbw / 2.0));   // :304-307
+    for (int j = 0; j < bbnfft; j++) bbcycbuff[j] = 0;                                          // :308
+}
+
 // ------------------------------------------------------------------ MSK
 MskDemodOracle::MskDemodOracle(const DemodSettings &st) : s(st)
 {
@@ -404,5 +417,16 @@ void MskDemodOracle::FreqOffsetEstimateSlot(double est)
     } else countdown = 4;
     if (mse > s.signalthreshold) n_sig_false++; else n_sig_true++;                              // :516-517
     if (on_sigstat) on_sigstat(hook_ctx, !(mse > s.signalthreshold));
+}
+
+void MskDemodOracle::CenterFreqChangedSlot(double freq_center)
+{
+    if (freq_center < (0.75 * s.fb)) freq_center = 0.75 * s.fb;                                 // :267-268
+    if (freq_center > (s.Fs / 2.0 - 0.75 * s.fb)) freq_center = s.Fs / 2.0 - 0.75 * s.fb;
+    mixer_center.SetFreq(freq_center, (int)s.Fs);                                               // :269
+    if (s.afc) mixer2.SetFreq(mixer_center.GetFreqHz());                                        // :270
+    if ((mixer2.GetFreqHz() - mixer_center.GetFreqHz()) > (s.lockingbw / 2.0)) mixer2.SetFreq(mixer_center.GetFreqHz() + (s.lockingbw / 2.0));    // :271-274
+    if ((mixer2.GetFreqHz() - mixer_center.GetFreqHz()) < (-s.lockingbw / 2.0)) mixer2.SetFreq(mixer_center.GetFreqHz() - (s.lockingbw / 2.0));   // :275-278
+    for (int j = 0; j < bbnfft; j++) bbcycbuff[j] = 0;                                          // :279
 }
 } // namespace jor

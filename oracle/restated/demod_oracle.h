@@ -42,7 +42,11 @@ struct OqpskDemodOracle                                // oqpskdemodulator.cpp
     explicit OqpskDemodOracle(const DemodSettings &);
     void writeData(const int16_t *pcm, long n);        // :334-627
     void FreqOffsetEstimateSlot(double est);           // :629-677
+    void CenterFreqChangedSlot(double freq_center);    // :291-310
     void DCDstatSlot(bool d) { dcd = d; }
+    void setAFC(bool v) { s.afc = v; }                 // :149-163
+    void setSQL(bool v) { s.sql = v; }
+    void setCPUReduce(bool v) { s.cpuReduce = v; }
 };
 
 struct MskDemodOracle                                  // mskdemodulator.cpp
@@ -59,7 +63,11 @@ struct MskDemodOracle                                  // mskdemodulator.cpp
     explicit MskDemodOracle(const DemodSettings &);
     void writeData(const int16_t *pcm, long n);        // :313-488
     void FreqOffsetEstimateSlot(double est);           // :490-519
+    void CenterFreqChangedSlot(double freq_center);    // :265-282
     void DCDstatSlot(bool d) { dcd = d; }
+    void setAFC(bool v) { s.afc = v; }                 // :105-122
+    void setSQL(bool v) { s.sql = v; }
+    void setCPUReduce(bool v) { s.cpuReduce = v; }
 };
 } // namespace jor
 #endif

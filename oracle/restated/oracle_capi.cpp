@@ -27,6 +27,15 @@ void jor_burst_set_sql(void *hv, int sql)          // burst OQPSK squelch (burst
 { OrHandle *h = (OrHandle *)hv; if (h->kind == 3) h->boq->sql = (sql != 0); }
 void jor_set_dcd(void *hv, int d)
 { OrHandle *h = (OrHandle *)hv; if (h->kind == 0) h->oq->DCDstatSlot(d != 0); else if (h->kind == 1) h->msk->DCDstatSlot(d != 0); else if (h->kind == 2) h->bmsk->dcd = (d != 0); }
+// CenterFreqChangedSlot / setAFC / setSQL / setCPUReduce of the continuous demodulators (kinds 0 and 1)
+void jor_set_center_freq(void *hv, double hz)
+{ OrHandle *h = (OrHandle *)hv; if (h->kind == 0) h->oq->CenterFreqChangedSlot(hz); else if (h->kind == 1) h->msk->CenterFreqChangedSlot(hz); }
+void jor_set_afc(void *hv, int v)
+{ OrHandle *h = (OrHandle *)hv; if (h->kind == 0) h->oq->setAFC(v != 0); else if (h->kind == 1) h->msk->setAFC(v != 0); }
+void jor_set_sql(void *hv, int v)
+{ OrHandle *h = (OrHandle *)hv; if (h->kind == 0) h->oq->setSQL(v != 0); else if (h->kind == 1) h->msk->setSQL(v != 0); }
+void jor_set_cpu_reduce(void *hv, int v)
+{ OrHandle *h = (OrHandle *)hv; if (h->kind == 0) h->oq->setCPUReduce(v != 0); else if (h->kind == 1) h->msk->setCPUReduce(v != 0); }
 static std::vector<short> &soft_of(OrHandle *h) { return h->kind == 0 ? h->oq->soft_out : (h->kind == 1 ? h->msk->soft_out : (h->kind == 2 ? h->bmsk->soft_out : h->boq->soft_out)); }
 long jor_soft_count(void *hv)
 { OrHandle *h = (OrHandle *)hv; return (long)soft_of(h).size(); }

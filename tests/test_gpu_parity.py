@@ -540,25 +540,40 @@ def test_c_channel_frames_on_reference_recording(golden):
             assert len(su) >= 5 and int(cok.sum()) >= 10
 
 
+def _tiny_writes_stream(name):
+    if name == "oqpsk_8000":                       # as test_oqpsk_parity_below_8400_bps
+        from jaero_b200 import synth
+        rng = np.random.default_rng(8000)
+        env = synth.oqpsk_envelope(rng.integers(0, 2, size=8000 * 3, dtype=np.uint8), 8000.0)
+        return synth.to_passband_int16(env, 6000.0, ebn0_db=12.0, fb=8000.0, rng=rng)
+    return load_excerpt(name)[:48000 * 3]
+
+
 @pytest.mark.parametrize("kind,name,kw", [
     ("oqpsk", "oqpsk_10500", dict(fb=10500, freq_center=5760, lockingbw=10500, fft_power=14, signalthreshold=0.65, afc=True)),
     ("msk", "msk_600", dict(fb=600, freq_center=1000, lockingbw=900, fft_power=13, signalthreshold=0.5, afc=True)),
+    ("oqpsk", "oqpsk_8400", dict(fb=8400, freq_center=8000, lockingbw=10500, fft_power=14, signalthreshold=0.65, afc=True)),
+    ("oqpsk", "oqpsk_8000", dict(fb=8000, freq_center=6000, lockingbw=8000, fft_power=14, signalthreshold=0.65, afc=True)),
+    ("msk", "msk_1200", dict(fb=1200, freq_center=2000, lockingbw=1800, fft_power=13, signalthreshold=0.5, afc=True)),
 ])
 def test_pipeline_kernels_with_tiny_and_odd_writes(kind, name, kw):
-    """The warp-specialised segment kernels hand samples between warps through named barriers; writes of 1, 2, 3 ... samples
-    (launches whose loop body runs 0, 1 or 2 times, estimator triggers on the first / last sample of a call) must give the
-    same stream as regular 4800-sample writes."""
+    """The segment kernels hand samples between warps through named barriers (10.5k, MSK) and between launches at every write
+    and estimator trigger; writes of 1, 2, 3 ... samples (launches whose loop body runs 0, 1 or 2 times, estimator triggers on
+    the first / last sample of a call) must give the oracle's stream for the same writes, and, where the reference does not
+    depend on the write boundaries, the same stream as regular 4800-sample writes. At 8400 bps it does: the pre-filter and its
+    mixer follow the writes (oqpskdemodulator.cpp:343-381,608)."""
     jb = _import()
-    pcm = load_excerpt(name)[:48000 * 3]
+    pcm = _tiny_writes_stream(name)
     pcm2 = np.stack([pcm, pcm[::-1].copy(), (pcm // 2).astype(np.int16)])
     ref, st_ref = _run_gpu(kind, pcm2, kw, 4800)
     b = jb.DemodBatch(kind, 3, **kw)
     acc = [[] for _ in range(3)]
     pattern = [1, 2, 3, 1, 5, 4093, 1, 1, 2, 4096, 7, 2047, 1, 2049, 31, 33, 4800, 64, 1]
+    writes = []
     a = 0; k = 0
     while a < pcm2.shape[1]:
         n = min(pattern[k % len(pattern)], pcm2.shape[1] - a)
-        b.write(pcm2[:, a:a + n]); a += n; k += 1
+        b.write(pcm2[:, a:a + n]); a += n; k += 1; writes.append(n)
         if k % 6 == 0:
             for c, s_ in enumerate(b.read_softbits()):
                 acc[c].append(s_)
@@ -566,10 +581,18 @@ def test_pipeline_kernels_with_tiny_and_odd_writes(kind, name, kw):
         acc[c].append(s_)
     st = b.status()
     b.close()
+    okw = dict(kw); okw.setdefault("fft_power", 14 if kind == "oqpsk" else 13)
     for c in range(3):
-        assert np.array_equal(np.concatenate(acc[c]), ref[c])
-        for key in ("mixer2_freq", "mixer2_wtptr", "st_wtptr", "mse", "agc"):
-            assert st[c][key] == st_ref[c][key], key
+        got = np.concatenate(acc[c])
+        d = restated.OracleDemod(kind, **okw)
+        a = 0
+        for n in writes:
+            d.write(pcm2[c, a:a + n]); a += n
+        _assert_parity(got, st[c], d.take_soft(), d.state())
+        if kw["fb"] != 8400:
+            assert np.array_equal(got, ref[c])
+            for key in ("mixer2_freq", "mixer2_wtptr", "st_wtptr", "mse", "agc"):
+                assert st[c][key] == st_ref[c][key], key
 
 
 def test_ingest_router_feeds_a_batch_like_direct_writes():

@@ -101,20 +101,27 @@ def _run_restated(case, pcm):
             d.write(pcm[a:a + case["chunk"]])
         return d.take_soft(), d.state(), np.zeros(0)
     d = restated.OracleDemod(case["kind"], **case["kw"])
-    sched = {int(a): int(v) for a, v in case["dcd_schedule"]}
-    for a in range(0, len(pcm), case["chunk"]):
-        if a in sched:
-            d.set_dcd(sched[a])
-        d.write(pcm[a:a + case["chunk"]])
+    # run-time control calls (tests/control_schedules.py) and the DCD schedule, each made before the write that starts there
+    events = [(int(a), [tuple(c) for c in calls]) for a, calls in case.get("controls", [])]
+    events += [(int(a), [("set_dcd", int(v))]) for a, v in case["dcd_schedule"]]
+    for a, n, calls in restated.write_plan(len(pcm), case["chunk"], events):
+        restated.apply_calls(d, calls)
+        d.write(pcm[a:a + n])
     return d.take_soft(), d.state(), d.take_cfe_log()
 
 
 @pytest.mark.parametrize("name", ["oqpsk_10500", "oqpsk_10500_noafc_dcd", "oqpsk_8400", "msk_600", "msk_1200", "msk_1200_noafc_dcd",
-                                  "burst_msk_1200_a", "burst_msk_1200_b", "burst_oqpsk_10500"])
+                                  "burst_msk_1200_a", "burst_msk_1200_b", "burst_oqpsk_10500",
+                                  "oqpsk_10500_controls", "oqpsk_8400_controls", "msk_600_controls", "msk_1200_controls"])
 def test_restated_oracle_matches_reference_golden(golden, name):
     """The restatement reproduces the verbatim reference bit for bit on the recordings (soft bits, coarse
-    estimates, loop state) — golden values were produced by oracle/_ref (tools/make_golden_outputs.py)."""
+    estimates, loop state) — golden values were produced by oracle/_ref (tools/make_golden_outputs.py). The *_controls
+    cases make the run-time control calls of tests/control_schedules.py between writes."""
     case = golden[name]
+    if "controls" in case:                                 # the committed schedule is the one the tests generate
+        import control_schedules
+        ev = control_schedules.events(control_schedules.recording_schedule(case["excerpt"], len(load_excerpt(case["excerpt"]))))
+        assert case["controls"] == [[a, [list(c) for c in calls]] for a, calls in ev]
     soft, state, cfe = _run_restated(case, load_excerpt(case["excerpt"]))
     assert len(soft) == case["n_soft"]
     assert hashlib.sha256(soft.astype("<i2").tobytes()).hexdigest() == case["soft_sha256"]

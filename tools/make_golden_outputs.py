@@ -14,7 +14,9 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
 from oracle import ref, restated  # noqa: E402
+import control_schedules  # noqa: E402
 
 CASES = {
     "oqpsk_10500": dict(kind="oqpsk", kw=dict(fb=10500, freq_center=5760, lockingbw=10500, fft_power=14, signalthreshold=0.65, afc=True)),
@@ -30,15 +32,19 @@ CASES = {
     "msk_1200_noafc_dcd": dict(kind="msk", excerpt="msk_1200", dcd_at=144000,
                                kw=dict(fb=1200, freq_center=2030, lockingbw=1800, fft_power=13, signalthreshold=0.5, afc=False)),
 }
+# the run-time controls (tests/control_schedules.py): the centre-change slot, AFC, squelch, CPU-reduce and DCD called between writes
+for _name, (_kind, _kw, _) in control_schedules.RECORDINGS.items():
+    CASES[_name + "_controls"] = dict(kind=_kind, excerpt=_name, kw=_kw, nosu=_kw["fb"] == 8400, controls=True)
 
 
 def run_case(name, case, chunk=4800):
     import multiprocessing as mp
     pcm = np.load(os.path.join(ROOT, "tests", "golden", case.get("excerpt", name) + "_excerpt.npz"))["pcm"]
     sched = [(case["dcd_at"], 1)] if "dcd_at" in case else None
+    controls = control_schedules.events(control_schedules.recording_schedule(case["excerpt"], len(pcm))) if case.get("controls") else []
     ctx = mp.get_context("spawn")            # fresh process: the reference keeps function-local statics
-    with ctx.Pool(1) as pool:
-        soft, state, cfe = pool.apply(ref.run_demod_job, ((case["kind"], case["kw"], pcm, chunk, sched),))
+    with ctx.Pool(1, maxtasksperchild=1) as pool:
+        soft, state, cfe = pool.apply(ref.run_demod_job, ((case["kind"], case["kw"], pcm, chunk, sched, controls),))
     if case.get("nosu"):
         su = np.zeros((0, 12), dtype=np.uint8); ok = np.zeros(0, dtype=np.int32); fr = np.zeros(0, dtype=np.int64)
     else:
@@ -65,6 +71,7 @@ def run_case(name, case, chunk=4800):
         "rt_packets": rt_packets,
         "kind": case["kind"], "kw": case["kw"], "excerpt": case.get("excerpt", name), "chunk": chunk,
         "dcd_schedule": sched or [],
+        **({"controls": [[int(a), [list(c) for c in calls]] for a, calls in controls]} if controls else {}),
         "n_soft": int(len(soft)), "soft_sha256": hashlib.sha256(soft.astype("<i2").tobytes()).hexdigest(),
         "soft_head": [int(x) for x in soft[:64]],
         "state": {k: float(v) for k, v in state.items()},
