@@ -250,6 +250,89 @@ def _p(a):
     return a.ctypes.data_as(ctypes.c_void_p)
 
 
+IQ_FORMATS = {"cu8": IQ_CU8, "cs16": IQ_CS16, IQ_CU8: IQ_CU8, IQ_CS16: IQ_CS16}
+
+
+def _iq_format(fmt):
+    """the JAERO_IQ_* code of an IQ format, given by name or code"""
+    if fmt not in IQ_FORMATS:
+        raise ValueError("IQ format is 'cu8' or 'cs16'")
+    return IQ_FORMATS[fmt]
+
+
+def _host_iq(iq, fmt):
+    """(contiguous interleaved host IQ, JAERO_IQ_* code) for a *_write: uint8 for 'cu8', int16 for 'cs16', an even count"""
+    f = _iq_format(fmt)
+    iq = np.ascontiguousarray(iq)
+    want = np.uint8 if f == IQ_CU8 else np.int16
+    if iq.dtype != want:
+        raise ValueError("%s IQ must be %s, got %s" % ("cu8" if f == IQ_CU8 else "cs16", np.dtype(want).name, iq.dtype))
+    if iq.size % 2:
+        raise ValueError("interleaved IQ needs an even number of values")
+    return iq, f
+
+
+def _pcm_rows(pcm, n_channels):
+    """(int16 host PCM [n_channels, n_samples] with unit-stride rows, row stride in samples) for a *_write"""
+    pcm = np.asarray(pcm)
+    if pcm.dtype != np.int16 or pcm.ndim != 2 or pcm.shape[0] != n_channels:
+        raise ValueError("pcm must be int16 [%d, n_samples]" % n_channels)
+    if pcm.strides[1] != 2 or pcm.strides[0] % 2:
+        pcm = np.ascontiguousarray(pcm)
+    return pcm, pcm.strides[0] // 2 if pcm.shape[0] > 1 else pcm.shape[1]
+
+
+class _Handle:
+    """A library object behind self.h: close() destroys it with jaero_<_NAME>_destroy, and so does garbage collection."""
+    _NAME = None
+
+    def close(self):
+        if self.h:
+            getattr(lib(), "jaero_%s_destroy" % self._NAME)(self.h); self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class _Stage(_Handle):
+    """The calls every front-end stage (Ddc, Resampler, Scanner, Identifier) has"""
+
+    def set_stream(self, cuda_stream):
+        _check(getattr(lib(), "jaero_%s_set_stream" % self._NAME)(self.h, ctypes.c_void_p(cuda_stream)))
+
+    @property
+    def launches(self):
+        return getattr(lib(), "jaero_%s_launch_count" % self._NAME)(self.h)
+
+
+class _PcmStage(_Stage):
+    """The output of the stages that produce n_channels rows of PCM per write (Ddc, Resampler)"""
+
+    def output(self):
+        """(device pointer, outputs per channel, row stride) of the PCM the last write produced"""
+        a, n, s = ctypes.c_void_p(), ctypes.c_size_t(), ctypes.c_size_t()
+        _check(getattr(lib(), "jaero_%s_output" % self._NAME)(self.h, ctypes.byref(a), ctypes.byref(n), ctypes.byref(s)))
+        return a.value, n.value, s.value
+
+    def read_pcm(self):
+        """host copy [n_channels, n] of the PCM the last write produced"""
+        _, n, _ = self.output()
+        out = np.zeros((self.n, max(n, 1)), dtype=np.int16)
+        got = ctypes.c_size_t()
+        _check(getattr(lib(), "jaero_%s_read_pcm" % self._NAME)(self.h, _p(out), out.shape[1], ctypes.byref(got)))
+        return out[:, :got.value]
+
+    def stats(self):
+        """(input samples per channel written, clipped output samples per channel)"""
+        n = ctypes.c_int64()
+        clipped = np.zeros(self.n, dtype=np.int64)
+        _check(getattr(lib(), "jaero_%s_get_stats" % self._NAME)(self.h, ctypes.byref(n), _p(clipped)))
+        return n.value, clipped
+
+
 def probe_fastfir(taps, x, nfft, writes, device=0):
     """test support: the streaming FFT convolution (include/jaero_b200.h, jaero_probe_fastfir) of x [n_channels, n] complex with
     taps [K] complex, fed as the write calls `writes` (sizes adding up to n). -> y [n_channels, n] complex"""
@@ -285,11 +368,12 @@ def probe_osc(op, arg, samplerate, device=0):
     return log
 
 
-class DemodBatch:
+class DemodBatch(_Handle):
     """n_channels independent continuous demodulators on one GPU (kind 'oqpsk' or 'msk').
 
     write() == the reference's writeData() for every channel; read_softbits() returns what the
     reference would have emitted through processDemodulatedSoftBits since the previous read."""
+    _NAME = "batch"
 
     def __init__(self, kind, n_channels, fb, Fs=48000.0, freq_center=8000.0, lockingbw=10500.0, fft_power=None,
                  signalthreshold=None, afc=False, sql=False, cpu_reduce=False, report_ebno=True, device=0):
@@ -412,19 +496,10 @@ class DemodBatch:
     def launches(self):
         return lib().jaero_batch_launch_count(self.h)
 
-    def close(self):
-        if self.h:
-            lib().jaero_batch_destroy(self.h); self.h = None
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-class ViterbiBatch:
+class ViterbiBatch(_Handle):
     """Batched JConvolutionalCodec (K=7, r=1/2, polys 109/79): Decode_Continuous / Decode_soft."""
+    _NAME = "viterbi"
 
     def __init__(self, n_channels, paddinglength=24, device=0):
         self.h = ctypes.c_void_p()
@@ -460,16 +535,6 @@ class ViterbiBatch:
     def launches(self):
         return lib().jaero_viterbi_launch_count(self.h)
 
-    def close(self):
-        if self.h:
-            lib().jaero_viterbi_destroy(self.h); self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
 
 def _pack_soft(n, soft_list):
     """per-channel soft-bit arrays -> (buf[n, cap] int16 zero-padded to the longest, cap, counts[n]) for *_process_softbits"""
@@ -481,8 +546,9 @@ def _pack_soft(n, soft_list):
     return buf, cap, counts
 
 
-class PChannelBatch:
+class PChannelBatch(_Handle):
     """Batched AeroL P-channel frame layer (600/1200/10500 bps, continuous): soft bits -> CRC-checked SUs + DCD."""
+    _NAME = "pchannel"
 
     def __init__(self, n_channels, fb, device=0):
         self.h = ctypes.c_void_p()
@@ -544,16 +610,6 @@ class PChannelBatch:
     def launches(self):
         return lib().jaero_pchannel_launch_count(self.h)
 
-    def close(self):
-        if self.h:
-            lib().jaero_pchannel_destroy(self.h); self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
 
 class BurstStatus(ctypes.Structure):
     _fields_ = [(n, ctypes.c_double) for n in
@@ -561,8 +617,9 @@ class BurstStatus(ctypes.Structure):
                  "rotator_freq", "n_sig_true", "n_sig_false", "cntr", "startstop", "last_burst_ebno", "n_ebno_emits")]
 
 
-class BurstMskBatch:
+class BurstMskBatch(_Handle):
     """n_channels independent burst MSK demodulators (BurstMskDemodulator, 600 / 1200 bps R/T channels)."""
+    _NAME = "burst"
 
     def __init__(self, n_channels, fb=1200.0, Fs=48000.0, freq_center=1000.0, lockingbw=1800.0, signalthreshold=0.6, device=0):
         if n_channels <= 0:
@@ -630,16 +687,6 @@ class BurstMskBatch:
     def launches(self):
         return lib().jaero_burst_launch_count(self.h)
 
-    def close(self):
-        if self.h:
-            lib().jaero_burst_destroy(self.h); self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
 
 class BurstOqpskBatch(BurstMskBatch):
     """n_channels independent burst OQPSK demodulators (BurstOqpskDemodulator, 10500 bps bursts)."""
@@ -654,8 +701,9 @@ class BurstOqpskBatch(BurstMskBatch):
         _check(lib().jaero_burst_oqpsk_create(ctypes.byref(s), n_channels, device, ctypes.byref(self.h)))
 
 
-class RTChannelBatch:
+class RTChannelBatch(_Handle):
     """R/T burst channel layer for n_channels streams: soft bits (with -1 start-of-burst markers) -> R / T packets."""
+    _NAME = "rt"
     RECORD = 400
 
     def __init__(self, n_channels, fb, device=0):
@@ -702,19 +750,10 @@ class RTChannelBatch:
     def launches(self):
         return lib().jaero_rt_launch_count(self.h)
 
-    def close(self):
-        if self.h:
-            lib().jaero_rt_destroy(self.h); self.h = None
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-class CChannelBatch:
+class CChannelBatch(_Handle):
     """C-channel (8400 bps) frame layer: soft bits -> per frame three sub-band signal units (+CRC) and 25 x 12 voice bytes."""
+    _NAME = "cchannel"
     RECORD = 352
 
     def __init__(self, n_channels, device=0):
@@ -763,19 +802,10 @@ class CChannelBatch:
     def launches(self):
         return lib().jaero_cchannel_launch_count(self.h)
 
-    def close(self):
-        if self.h:
-            lib().jaero_cchannel_destroy(self.h); self.h = None
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-class IngestRouter:
+class IngestRouter(_Handle):
     """ZMQ-style [topic][uint32 rate][int16 PCM] messages -> per-channel staging -> DemodBatch.write (host side, no libzmq)."""
+    _NAME = "ingest"
 
     def __init__(self, topics, sample_rate=48000, capacity_samples=192000):
         self.n = len(topics)
@@ -802,20 +832,11 @@ class IngestRouter:
         _check(lib().jaero_ingest_flush(self.h, batch.h, n))
         return n
 
-    def close(self):
-        if self.h:
-            lib().jaero_ingest_destroy(self.h); self.h = None
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-class Reassembler:
+class Reassembler(_Handle):
     """Per-channel ISU/SSU reassembly + ACARS parsing + defragmentation (host side; mirrors the reference's ISUData,
     RISUData, ParserISU and ACARSDefragmenter, JAERO/aerol.cpp:4-487). Feed CRC-valid signal units only."""
+    _NAME = "reasm"
 
     COMPLETE, MISSING, PARSED = 1, 2, 4
 
@@ -874,16 +895,6 @@ class Reassembler:
         _check(lib().jaero_reasm_get_stats(self.h, a, a + 8, a + 16, a + 24))
         return dict(isus=v[0], messages=v[1], errors=v[2], missing=v[3])
 
-    def close(self):
-        if self.h:
-            lib().jaero_reasm_destroy(self.h); self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
 
 def ddc_plan(input_rate, decimation, bandwidth, transition, interpolation=1):
     """The down-converter's filter stages for a set-up (host only, no device): dict(L, D1, K1, D2, K2, h1, h2), output rate
@@ -909,11 +920,12 @@ def rate_ratio(input_rate, output_rate=48000.0):
     return q.numerator, q.denominator
 
 
-class Ddc:
+class Ddc(_PcmStage):
     """Wideband IQ digital down-converter (include/jaero_b200.h, jaero_ddc_*): one cu8 / cs16 IQ stream at input_rate ->
     n_channels real int16 PCM streams at output_rate = input_rate * interpolation / decimation, channel c tuned to offsets_hz[c]
     and placed at audio_hz[c]. rate_ratio gives (interpolation, decimation) for a radio's rate."""
-    FORMATS = {"cu8": IQ_CU8, "cs16": IQ_CS16, IQ_CU8: IQ_CU8, IQ_CS16: IQ_CS16}
+    _NAME = "ddc"
+    FORMATS, _iq = IQ_FORMATS, staticmethod(_host_iq)                 # the IQ formats and host-IQ check of every stage
 
     def __init__(self, input_rate, decimation, offsets_hz, audio_hz, bandwidth, transition, gain=1.0, device=0, interpolation=1):
         off = np.ascontiguousarray(offsets_hz, dtype=np.float64).reshape(-1)
@@ -928,72 +940,20 @@ class Ddc:
                                                float(bandwidth), float(transition), float(gain), device, ctypes.byref(self.h)))
         self.plan = ddc_plan(input_rate, decimation, bandwidth, transition, interpolation)
 
-    @staticmethod
-    def _iq(iq, fmt):
-        if fmt not in Ddc.FORMATS:
-            raise ValueError("IQ format is 'cu8' or 'cs16'")
-        f = Ddc.FORMATS[fmt]
-        iq = np.ascontiguousarray(iq)
-        want = np.uint8 if f == IQ_CU8 else np.int16
-        if iq.dtype != want:
-            raise ValueError("%s IQ must be %s, got %s" % ("cu8" if f == IQ_CU8 else "cs16", np.dtype(want).name, iq.dtype))
-        if iq.size % 2:
-            raise ValueError("interleaved IQ needs an even number of values")
-        return iq, f
-
     def write(self, iq, fmt):
         """iq: interleaved I, Q (uint8 for 'cu8', int16 for 'cs16'), host memory"""
-        iq, f = self._iq(iq, fmt)
+        iq, f = _host_iq(iq, fmt)
         _check(lib().jaero_ddc_write(self.h, _p(iq), iq.size // 2, f))
 
     def write_device(self, dev_ptr, n_iq, fmt):
-        if fmt not in self.FORMATS:
-            raise ValueError("IQ format is 'cu8' or 'cs16'")
-        _check(lib().jaero_ddc_write_device(self.h, ctypes.c_void_p(dev_ptr), int(n_iq), self.FORMATS[fmt]))
-
-    def output(self):
-        """(device pointer, outputs per channel, row stride) of the PCM the last write produced"""
-        a, n, s = ctypes.c_void_p(), ctypes.c_size_t(), ctypes.c_size_t()
-        _check(lib().jaero_ddc_output(self.h, ctypes.byref(a), ctypes.byref(n), ctypes.byref(s)))
-        return a.value, n.value, s.value
-
-    def read_pcm(self):
-        """host copy [n_channels, n] of the PCM the last write produced"""
-        _, n, _ = self.output()
-        out = np.zeros((self.n, max(n, 1)), dtype=np.int16)
-        got = ctypes.c_size_t()
-        _check(lib().jaero_ddc_read_pcm(self.h, _p(out), out.shape[1], ctypes.byref(got)))
-        return out[:, :got.value]
-
-    def set_stream(self, cuda_stream):
-        _check(lib().jaero_ddc_set_stream(self.h, ctypes.c_void_p(cuda_stream)))
+        f = _iq_format(fmt)
+        _check(lib().jaero_ddc_write_device(self.h, ctypes.c_void_p(dev_ptr), int(n_iq), f))
 
     def set_offset(self, hz, channel=-1):
         _check(lib().jaero_ddc_set_offset(self.h, channel, float(hz)))
 
     def set_audio_freq(self, hz, channel=-1):
         _check(lib().jaero_ddc_set_audio_freq(self.h, channel, float(hz)))
-
-    def stats(self):
-        """(input samples written, clipped output samples per channel)"""
-        n = ctypes.c_int64()
-        clipped = np.zeros(self.n, dtype=np.int64)
-        _check(lib().jaero_ddc_get_stats(self.h, ctypes.byref(n), _p(clipped)))
-        return n.value, clipped
-
-    @property
-    def launches(self):
-        return lib().jaero_ddc_launch_count(self.h)
-
-    def close(self):
-        if self.h:
-            lib().jaero_ddc_destroy(self.h); self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 def resample_plan(input_rate, output_rate, passband_hz):
@@ -1007,9 +967,10 @@ def resample_plan(input_rate, output_rate, passband_hz):
     return dict(L=int(st[0]), M=int(st[1]), K=int(st[2]), h=h)
 
 
-class Resampler:
+class Resampler(_PcmStage):
     """PCM rate converter (include/jaero_b200.h, jaero_resample_*): n_channels int16 PCM streams at input_rate -> int16 PCM at
     output_rate (the demodulators' 48 kHz by default), on the device. passband_hz defaults to 0.45 min(input_rate, output_rate)."""
+    _NAME = "resample"
 
     def __init__(self, input_rate, n_channels, output_rate=48000, passband_hz=None, device=0):
         if n_channels <= 0:
@@ -1024,60 +985,18 @@ class Resampler:
 
     def write(self, pcm):
         """pcm: int16 array [n_channels, n_samples] (host); rows may be strided"""
-        pcm = np.asarray(pcm)
-        if pcm.dtype != np.int16 or pcm.ndim != 2 or pcm.shape[0] != self.n:
-            raise ValueError("pcm must be int16 [%d, n_samples]" % self.n)
-        if pcm.strides[1] != 2 or pcm.strides[0] % 2:
-            pcm = np.ascontiguousarray(pcm)
-        stride = pcm.strides[0] // 2 if pcm.shape[0] > 1 else pcm.shape[1]
+        pcm, stride = _pcm_rows(pcm, self.n)
         _check(lib().jaero_resample_write(self.h, _p(pcm), pcm.shape[1], stride))
 
     def write_device(self, dev_ptr, n_samples, stride):
         """the same from a DEVICE buffer [n_channels][stride] int16"""
         _check(lib().jaero_resample_write_device(self.h, ctypes.c_void_p(dev_ptr), int(n_samples), int(stride)))
 
-    def output(self):
-        """(device pointer, outputs per channel, row stride) of the PCM the last write produced"""
-        a, n, s = ctypes.c_void_p(), ctypes.c_size_t(), ctypes.c_size_t()
-        _check(lib().jaero_resample_output(self.h, ctypes.byref(a), ctypes.byref(n), ctypes.byref(s)))
-        return a.value, n.value, s.value
 
-    def read_pcm(self):
-        """host copy [n_channels, n] of the PCM the last write produced"""
-        _, n, _ = self.output()
-        out = np.zeros((self.n, max(n, 1)), dtype=np.int16)
-        got = ctypes.c_size_t()
-        _check(lib().jaero_resample_read_pcm(self.h, _p(out), out.shape[1], ctypes.byref(got)))
-        return out[:, :got.value]
-
-    def set_stream(self, cuda_stream):
-        _check(lib().jaero_resample_set_stream(self.h, ctypes.c_void_p(cuda_stream)))
-
-    def stats(self):
-        """(input samples per channel written, clipped output samples per channel)"""
-        n = ctypes.c_int64()
-        clipped = np.zeros(self.n, dtype=np.int64)
-        _check(lib().jaero_resample_get_stats(self.h, ctypes.byref(n), _p(clipped)))
-        return n.value, clipped
-
-    @property
-    def launches(self):
-        return lib().jaero_resample_launch_count(self.h)
-
-    def close(self):
-        if self.h:
-            lib().jaero_resample_destroy(self.h); self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-class Scanner:
+class Scanner(_Stage):
     """Wideband carrier scanner (include/jaero_b200.h, jaero_scan_*): the averaged and max-held power spectrum of one cu8 / cs16 IQ
     stream at input_rate, nfft bins in fftshift order, frames every `hop` samples (default nfft // 2)."""
+    _NAME = "scan"
 
     def __init__(self, input_rate, nfft, hop=None, device=0):
         self.input_rate, self.nfft = float(input_rate), int(nfft)
@@ -1087,13 +1006,12 @@ class Scanner:
 
     def write(self, iq, fmt):
         """iq: interleaved I, Q (uint8 for 'cu8', int16 for 'cs16'), host memory"""
-        iq, f = Ddc._iq(iq, fmt)
+        iq, f = _host_iq(iq, fmt)
         _check(lib().jaero_scan_write(self.h, _p(iq), iq.size // 2, f))
 
     def write_device(self, dev_ptr, n_iq, fmt):
-        if fmt not in Ddc.FORMATS:
-            raise ValueError("IQ format is 'cu8' or 'cs16'")
-        _check(lib().jaero_scan_write_device(self.h, ctypes.c_void_p(dev_ptr), int(n_iq), Ddc.FORMATS[fmt]))
+        f = _iq_format(fmt)
+        _check(lib().jaero_scan_write_device(self.h, ctypes.c_void_p(dev_ptr), int(n_iq), f))
 
     def reset(self):
         _check(lib().jaero_scan_reset(self.h))
@@ -1107,23 +1025,6 @@ class Scanner:
     def freqs(self):
         """frequency of each bin, Hz from the tuner centre"""
         return (np.arange(self.nfft) - self.nfft // 2) * (self.input_rate / self.nfft)
-
-    def set_stream(self, cuda_stream):
-        _check(lib().jaero_scan_set_stream(self.h, ctypes.c_void_p(cuda_stream)))
-
-    @property
-    def launches(self):
-        return lib().jaero_scan_launch_count(self.h)
-
-    def close(self):
-        if self.h:
-            lib().jaero_scan_destroy(self.h); self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 def find_carriers(psd, input_rate, threshold_db=3.0, floor_window_hz=100e3, floor_quantile=0.25, min_width_hz=200.0, dc_guard_hz=0.0):
@@ -1181,10 +1082,11 @@ def channel_plan(carriers, input_rate, decimation, interpolation=1):
     return out, unplanned
 
 
-class Identifier:
+class Identifier(_Stage):
     """Mode identifier (include/jaero_b200.h, jaero_ident_*): per channel of n_channels int16 PCM streams at Fs, the averaged power
     spectrum of the squared analytic signal, nfft bins in fftshift order, frames every nfft // 2 samples. identify() finds the
     JAERO bit rate and the carrier in one row of it."""
+    _NAME = "ident"
 
     def __init__(self, Fs, n_channels, nfft=16384, device=0):
         self.Fs, self.n, self.nfft = float(Fs), int(n_channels), int(nfft)
@@ -1193,12 +1095,7 @@ class Identifier:
 
     def write(self, pcm):
         """pcm: int16 array [n_channels, n_samples] (host); rows may be strided"""
-        pcm = np.asarray(pcm)
-        if pcm.dtype != np.int16 or pcm.ndim != 2 or pcm.shape[0] != self.n:
-            raise ValueError("pcm must be int16 [%d, n_samples]" % self.n)
-        if pcm.strides[1] != 2 or pcm.strides[0] % 2:
-            pcm = np.ascontiguousarray(pcm)
-        stride = pcm.strides[0] // 2 if pcm.shape[0] > 1 else pcm.shape[1]
+        pcm, stride = _pcm_rows(pcm, self.n)
         _check(lib().jaero_ident_write(self.h, _p(pcm), pcm.shape[1], stride))
 
     def write_device(self, dev_ptr, n_samples, stride):
@@ -1217,23 +1114,6 @@ class Identifier:
     def freqs(self):
         """frequency of each bin, Hz of the squared signal (twice the PCM frequency, modulo Fs)"""
         return (np.arange(self.nfft) - self.nfft // 2) * (self.Fs / self.nfft)
-
-    def set_stream(self, cuda_stream):
-        _check(lib().jaero_ident_set_stream(self.h, ctypes.c_void_p(cuda_stream)))
-
-    @property
-    def launches(self):
-        return lib().jaero_ident_launch_count(self.h)
-
-    def close(self):
-        if self.h:
-            lib().jaero_ident_destroy(self.h); self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 IDENT_MODES = ("msk600", "msk1200", "oqpsk8400", "oqpsk10500")     # the order of jaero_ident_result.score_db
@@ -1274,11 +1154,9 @@ def probe_carriers(carriers, input_rate, iq, fmt, interpolation=1, decimation=No
     out_rate = float(input_rate) * int(interpolation) / int(decimation)
     if isinstance(iq, tuple):
         dev_ptr, n_iq = int(iq[0]), int(iq[1])
-        if fmt not in Ddc.FORMATS:
-            raise ValueError("IQ format is 'cu8' or 'cs16'")
-        iq_bytes = 2 if Ddc.FORMATS[fmt] == IQ_CU8 else 4
+        iq_bytes = 2 if _iq_format(fmt) == IQ_CU8 else 4
     else:
-        dev_ptr, (iq, _) = None, Ddc._iq(iq, fmt)
+        dev_ptr, (iq, _) = None, _host_iq(iq, fmt)
         n_iq = iq.size // 2
     if seconds is not None:
         n_iq = min(n_iq, int(round(float(seconds) * float(input_rate))))

@@ -60,6 +60,22 @@ template <class T> struct CreateGuard {
     CreateGuard &operator=(const CreateGuard &) = delete;
 };
 
+// *_sync: waits for the object's queued work
+template <class O> int sync_stream(O *o)
+{
+    if (!o) { set_error("null handle"); return JAERO_E_ARG; }
+    JB_CUDA(cudaSetDevice(o->device));
+    JB_CUDA(cudaStreamSynchronize(o->stream));
+    return JAERO_OK;
+}
+// *_set_stream: the work queued on the old stream drains first; a null stream goes back to the object's own
+template <class O> int switch_stream(O *o, void *cuda_stream)
+{
+    int r = sync_stream(o); if (r) return r;
+    o->stream = cuda_stream ? (cudaStream_t)cuda_stream : o->own_stream;
+    return JAERO_OK;
+}
+
 struct jaero_viterbi {
     int n_channels, pad, device;
     cudaStream_t stream;
@@ -113,13 +129,7 @@ int jaero_viterbi_reset(jaero_viterbi *v)
     JB_CUDA(cudaMemsetAsync(v->d_overlap_len, 0, (size_t)v->n_channels * sizeof(int), v->stream));
     return JAERO_OK;
 }
-int jaero_viterbi_sync(jaero_viterbi *v)
-{
-    if (!v) { set_error("null handle"); return JAERO_E_ARG; }
-    JB_CUDA(cudaSetDevice(v->device));
-    JB_CUDA(cudaStreamSynchronize(v->stream));
-    return JAERO_OK;
-}
+int jaero_viterbi_sync(jaero_viterbi *v) { return sync_stream(v); }
 int64_t jaero_viterbi_launch_count(const jaero_viterbi *v) { return v ? v->launches : 0; }
 
 static int vit_check(jaero_viterbi *v, size_t n_soft, int cols)
@@ -800,14 +810,7 @@ void jaero_batch_destroy(jaero_batch *b)
 int jaero_batch_channels(const jaero_batch *b) { return b ? b->p.n_channels : 0; }
 int64_t jaero_batch_launch_count(const jaero_batch *b) { return b ? b->launches : 0; }
 
-int jaero_batch_set_stream(jaero_batch *b, void *cuda_stream)
-{
-    if (!b) { set_error("null handle"); return JAERO_E_ARG; }
-    JB_CUDA(cudaSetDevice(b->device));
-    JB_CUDA(cudaStreamSynchronize(b->stream));
-    b->stream = cuda_stream ? (cudaStream_t)cuda_stream : b->own_stream;
-    return JAERO_OK;
-}
+int jaero_batch_set_stream(jaero_batch *b, void *cuda_stream) { return switch_stream(b, cuda_stream); }
 int jaero_batch_set_profiling(jaero_batch *b, int enabled)
 {
     if (!b) { set_error("null handle"); return JAERO_E_ARG; }
@@ -983,13 +986,7 @@ int jaero_probe_osc(int device, int n_lanes, int n_ops, const int32_t *op, const
     return JAERO_OK;
 }
 
-int jaero_batch_sync(jaero_batch *b)
-{
-    if (!b) { set_error("null handle"); return JAERO_E_ARG; }
-    JB_CUDA(cudaSetDevice(b->device));
-    JB_CUDA(cudaStreamSynchronize(b->stream));
-    return JAERO_OK;
-}
+int jaero_batch_sync(jaero_batch *b) { return sync_stream(b); }
 
 int jaero_batch_write_device(jaero_batch *b, const int16_t *d_pcm, size_t n, size_t stride)
 {
@@ -1691,13 +1688,7 @@ void jaero_burst_destroy(jaero_burst *b)
     release(b, {b->d_stage}, {b->h_ints, b->h_dbls, b->h_soft}, b->stream);
 }
 int64_t jaero_burst_launch_count(const jaero_burst *b) { return b ? b->launches : 0; }
-int jaero_burst_sync(jaero_burst *b)
-{
-    if (!b) { set_error("null handle"); return JAERO_E_ARG; }
-    JB_CUDA(cudaSetDevice(b->device));
-    JB_CUDA(cudaStreamSynchronize(b->stream));
-    return JAERO_OK;
-}
+int jaero_burst_sync(jaero_burst *b) { return sync_stream(b); }
 int jaero_burst_write_device(jaero_burst *b, const int16_t *d_pcm, size_t n, size_t stride)
 {
     if (!b || !d_pcm) { set_error("jaero_burst_write_device: null argument"); return JAERO_E_ARG; }
@@ -2182,18 +2173,173 @@ static void ddc_design(double fs, double B, double dT, const DdcPlan &c, double 
 // round(f / fs * 2^32) mod 2^32
 static uint32_t tuning_word(double f, double fs) { return (uint32_t)(uint64_t)llround(f / fs * 4294967296.0); }
 
-struct jaero_ddc {
+// ------------------------------------------------------------------ host plumbing of the front-end stages
+// What the down-converter, the rate converter, the scanner and the identifier share: a device and a stream that set_stream can
+// replace, owned buffers, and the samples (per channel) taken and kernels launched since create.
+struct Stage {
     int device; cudaStream_t stream, own_stream;
     std::vector<void *> allocs;
+    long long n_in, launches;
+};
+// The down-converter's and the rate converter's output: the [n_channels][pcm_stride] PCM rows of the last write
+struct PcmStage : Stage {
+    int16_t *d_pcm; size_t pcm_cap, pcm_n, pcm_stride;
+};
+
+// The whole of a stage's destroy, for a non-null o: its queued work drains, then everything it owns is freed
+template <class O> void destroy_stage(O *o, std::initializer_list<void *> grown)
+{
+    cudaSetDevice(o->device);
+    cudaStreamSynchronize(o->stream);
+    release(o, grown, {}, o->own_stream);
+}
+
+static const size_t MAX_WRITE_SAMPLES = (size_t)1 << 34;
+static int arg_error(const char *fn, const char *what) { set_error(std::string(fn) + ": " + what); return JAERO_E_ARG; }
+static size_t iq_sample_bytes(int format) { return format == JAERO_IQ_CU8 ? 2 : 4; }
+
+// Argument checks of an IQ write, in this order: null handle or buffer, format, alignment to one sample (device buffers only), length
+static int iq_write_args(const void *o, const void *iq, size_t n, int format, bool device, const char *fn)
+{
+    if (!o || !iq) return arg_error(fn, "null argument");
+    if (format != JAERO_IQ_CU8 && format != JAERO_IQ_CS16) return arg_error(fn, "unknown IQ format");
+    if (device && ((uintptr_t)iq & (iq_sample_bytes(format) - 1))) return arg_error(fn, "IQ pointer not aligned to one sample");
+    if (n > MAX_WRITE_SAMPLES) return arg_error(fn, "too many samples in one write");
+    return JAERO_OK;
+}
+// Argument checks of a [n_channels][stride] PCM write, in this order: null handle or buffer, alignment to one sample (device
+// buffers only), stride, length
+static int pcm_write_args(const void *o, const int16_t *pcm, size_t n, size_t stride, bool device, const char *fn)
+{
+    if (!o || !pcm) return arg_error(fn, "null argument");
+    if (device && ((uintptr_t)pcm & 1)) return arg_error(fn, "PCM pointer not aligned to one sample");
+    if (stride < n) return arg_error(fn, "channel stride is smaller than n_samples");
+    if (n > MAX_WRITE_SAMPLES) return arg_error(fn, "too many samples in one write");
+    return JAERO_OK;
+}
+
+// A host IQ write: the bytes are staged in o->d_raw, then written as from the device. The copy is waited for, so the caller may
+// reuse its pageable buffer on return.
+template <class O> int stage_iq_write(O *o, const void *iq, size_t n, int format, const char *fn, int (*write_device)(O *, const void *, size_t, int))
+{
+    int r = iq_write_args(o, iq, n, format, false, fn); if (r) return r;
+    JB_CUDA(cudaSetDevice(o->device));
+    const size_t bytes = n * iq_sample_bytes(format);
+    if (grow((uint8_t **)&o->d_raw, &o->raw_cap, std::max<size_t>(bytes, 4), o->stream)) return JAERO_E_CUDA;
+    if (bytes) {
+        JB_CUDA(cudaMemcpyAsync(o->d_raw, iq, bytes, cudaMemcpyHostToDevice, o->stream));
+        JB_CUDA(cudaStreamSynchronize(o->stream));
+    }
+    return write_device(o, o->d_raw, n, format);
+}
+// A host PCM write: the rows are staged densely in o->d_in, [n_channels][n], then written as from the device, as above
+template <class O> int stage_pcm_write(O *o, const int16_t *pcm, size_t n, size_t stride, const char *fn,
+                                       int (*write_device)(O *, const int16_t *, size_t, size_t))
+{
+    int r = pcm_write_args(o, pcm, n, stride, false, fn); if (r) return r;
+    JB_CUDA(cudaSetDevice(o->device));
+    const size_t C = (size_t)o->p.n_channels;
+    if (grow(&o->d_in, &o->in_cap, std::max<size_t>(C * n, 1), o->stream)) return JAERO_E_CUDA;
+    if (n) {
+        JB_CUDA(cudaMemcpy2DAsync(o->d_in, n * sizeof(int16_t), pcm, stride * sizeof(int16_t), n * sizeof(int16_t), C, cudaMemcpyHostToDevice,
+                                  o->stream));
+        JB_CUDA(cudaStreamSynchronize(o->stream));
+    }
+    return write_device(o, o->d_in, n, n);
+}
+
+// Outputs m of an L/D rate change with floor(m D / L) in [n0, n0 + n): ceil((n0 + n) L / D) - ceil(n0 L / D)
+static size_t rational_outputs(long long n0, long long n, long long L, long long D) { return (size_t)(((n0 + n) * L + D - 1) / D - (n0 * L + D - 1) / D); }
+// 16-byte output rows: jaero_batch_write_device reads them in place
+static size_t pcm_row_stride(size_t m) { return std::max<size_t>(8, (m + 7) & ~(size_t)7); }
+
+// [L][R] per-phase taps of a K-tap prototype, hp[phi][r] = h[phi + r L], zero past its end
+static std::vector<double> polyphase_fold(const double *h, int K, int L, int R)
+{
+    std::vector<double> hp((size_t)L * R, 0.0);
+    for (int k = 0; k < K; k++) hp[(size_t)(k % L) * R + k / L] = h[k];
+    return hp;
+}
+
+template <class O> int pcm_output(O *o, const int16_t **d_pcm, size_t *n, size_t *stride, const char *fn)
+{
+    if (!o || !d_pcm || !n || !stride) return arg_error(fn, "null argument");
+    *d_pcm = o->d_pcm; *n = o->pcm_n; *stride = o->pcm_stride;
+    return JAERO_OK;
+}
+template <class O> int pcm_read(O *o, int16_t *out, size_t cap, size_t *n, const char *fn)
+{
+    if (!o || !out || !n) return arg_error(fn, "null argument");
+    if (cap < o->pcm_n) return arg_error(fn, "cap_per_channel is smaller than the last write's output");
+    JB_CUDA(cudaSetDevice(o->device));
+    if (o->pcm_n)
+        JB_CUDA(cudaMemcpy2DAsync(out, cap * sizeof(int16_t), o->d_pcm, o->pcm_stride * sizeof(int16_t), o->pcm_n * sizeof(int16_t),
+                                  o->p.n_channels, cudaMemcpyDeviceToHost, o->stream));
+    JB_CUDA(cudaStreamSynchronize(o->stream));
+    *n = o->pcm_n;
+    return JAERO_OK;
+}
+template <class O> int pcm_stats(O *o, int64_t *inputs, int64_t *clipped)
+{
+    if (!o) { set_error("null handle"); return JAERO_E_ARG; }
+    if (inputs) *inputs = o->n_in;
+    if (clipped) {
+        JB_CUDA(cudaSetDevice(o->device));
+        JB_CUDA(cudaMemcpyAsync(clipped, o->p.clipped, o->p.n_channels * sizeof(int64_t), cudaMemcpyDeviceToHost, o->stream));
+        JB_CUDA(cudaStreamSynchronize(o->stream));
+    }
+    return JAERO_OK;
+}
+
+// nfft of the scanner (max_nfft 65536) and the identifier (16384): a power of two from 1024
+static bool pow2_nfft(int nfft, int max_nfft) { return nfft >= 1024 && nfft <= max_nfft && (nfft & (nfft - 1)) == 0; }
+
+// The tables of a windowed four-step FFT of nfft points, in two owned buffers: the n1 x n2 split (n1 = 2^floor(log2(nfft) / 2)),
+// the twiddles W_N^k and the periodic Hann window. Returns the window's sum of squares in *wss.
+template <class O, class P> int four_step_tables(O *o, P &p, int nfft, double *wss)
+{
+    int lg = 0;
+    while ((1 << lg) < nfft) lg++;
+    p.n1 = 1 << (lg / 2); p.n2 = nfft / p.n1;
+    const std::vector<std::complex<double>> tw = twiddles(nfft);
+    std::vector<double> win(nfft);
+    *wss = 0.0;
+    for (int k = 0; k < nfft; k++) {
+        win[k] = 0.5 - 0.5 * tw[k].real();
+        *wss += win[k] * win[k];
+    }
+    double2 *dtw; double *dwin;
+    if (owned_alloc(o, &dtw, (size_t)nfft) || owned_alloc(o, &dwin, (size_t)nfft)) return JAERO_E_CUDA;
+    p.tw = dtw; p.win = dwin;
+    JB_CUDA(cudaMemcpyAsync(dtw, tw.data(), nfft * sizeof(double2), cudaMemcpyHostToDevice, o->stream));
+    JB_CUDA(cudaMemcpyAsync(dwin, win.data(), nfft * sizeof(double), cudaMemcpyHostToDevice, o->stream));
+    JB_CUDA(cudaStreamSynchronize(o->stream));                       // the tables are in place, the host vectors may go
+    return JAERO_OK;
+}
+
+// The frames a write of n samples completes, for a stage that has taken n_in samples and completed `frames` frames of N samples
+// every hop. The write's samples and the carry sit at x0 + j: the carry is the n_in - x0 samples from the first incomplete frame.
+struct FrameSpan {
+    long long total, x0, carry, f_end, F, x1;                       // x1: the first sample an incomplete frame needs after the write
+};
+static FrameSpan frame_span(long long n_in, long long frames, long long N, long long hop, size_t n)
+{
+    FrameSpan s;
+    s.total = n_in + (long long)n;
+    s.x0 = frames * hop; s.carry = n_in - s.x0;
+    s.f_end = s.total >= N ? (s.total - N) / hop + 1 : 0; s.F = s.f_end - frames;
+    s.x1 = s.f_end * hop;
+    return s;
+}
+
+struct jaero_ddc : PcmStage {
     DdcParams p;
     double fs_in, fs_out, B;
     std::vector<double> h1;                                          // host copy, for re-folding on set_offset
     std::vector<uint32_t> T, S;
     std::vector<double2> h1c;                                        // [K1][cpad] staging for the folded taps
-    long long n_in, launches;
     void *d_raw; size_t raw_cap;                                     // host writes: the IQ bytes staged on the device
     double2 *d_x, *d_u; size_t x_cap, u_cap;
-    int16_t *d_pcm; size_t pcm_cap, pcm_n, pcm_stride;
 };
 
 // Retunes are ordered on the DDC's stream like its kernels: writes queued before a retune read the old values, writes after it the
@@ -2276,8 +2422,7 @@ static int ddc_create(double input_rate, int L, int M, int n_channels, const dou
     d->h1.resize(c.K1);
     std::vector<double> h2(c.K2);
     ddc_design(input_rate, bandwidth, transition, c, d->h1.data(), h2.data());
-    std::vector<double> h2p((size_t)c.L * p.R, 0.0);                 // [L][R] per-phase taps, h2p[phi][r] = h2[phi + r L]
-    for (int k = 0; k < c.K2; k++) h2p[(size_t)(k % c.L) * p.R + k / c.L] = h2[k];
+    const std::vector<double> h2p = polyphase_fold(h2.data(), c.K2, c.L, p.R);
     d->T.resize(n_channels); d->S.resize(n_channels);
     for (int ch = 0; ch < n_channels; ch++) { d->T[ch] = tuning_word(offset_hz[ch], input_rate); d->S[ch] = tuning_word(audio_hz[ch], fs_out); }
     d->h1c.assign((size_t)c.K1 * p.cpad, make_double2(0.0, 0.0));
@@ -2317,28 +2462,17 @@ int jaero_ddc_create_rational(double input_rate, int interpolation, int decimati
     return ddc_create(input_rate, interpolation, decimation, n_channels, offset_hz, audio_hz, bandwidth, transition, gain, device, out,
                       "jaero_ddc_create_rational");
 }
-void jaero_ddc_destroy(jaero_ddc *d)
-{
-    if (!d) return;
-    cudaSetDevice(d->device);
-    cudaStreamSynchronize(d->stream);
-    release(d, {d->d_raw, d->d_x, d->d_u, d->d_pcm}, {}, d->own_stream);
-}
+void jaero_ddc_destroy(jaero_ddc *d) { if (d) destroy_stage(d, {d->d_raw, d->d_x, d->d_u, d->d_pcm}); }
 int64_t jaero_ddc_launch_count(const jaero_ddc *d) { return d ? d->launches : 0; }
 
 int jaero_ddc_write_device(jaero_ddc *d, const void *d_iq, size_t n, int format)
 {
-    if (!d || !d_iq) { set_error("jaero_ddc_write_device: null argument"); return JAERO_E_ARG; }
-    if (format != JAERO_IQ_CU8 && format != JAERO_IQ_CS16) { set_error("jaero_ddc_write_device: unknown IQ format"); return JAERO_E_ARG; }
-    if ((uintptr_t)d_iq & (format == JAERO_IQ_CU8 ? 1 : 3)) { set_error("jaero_ddc_write_device: IQ pointer not aligned to one sample"); return JAERO_E_ARG; }
-    if (n > ((size_t)1 << 34)) { set_error("jaero_ddc_write_device: too many samples in one write"); return JAERO_E_ARG; }
+    int r = iq_write_args(d, d_iq, n, format, true, "jaero_ddc_write_device"); if (r) return r;
     JB_CUDA(cudaSetDevice(d->device));
     DdcParams &p = d->p;
-    const long long n0 = d->n_in, D = (long long)p.D1 * p.D2;
-    // outputs m with floor(m D / L) in [n0, n0 + n): ceil((n0 + n) L / D) - ceil(n0 L / D)
-    const size_t M = (size_t)(((n0 + (long long)n) * p.L + D - 1) / D - (n0 * p.L + D - 1) / D);
-    const size_t J = (size_t)((n0 + (long long)n + p.D1 - 1) / p.D1 - (n0 + p.D1 - 1) / p.D1);
-    const size_t stride = std::max<size_t>(8, (M + 7) & ~(size_t)7);   // 16-byte rows: jaero_batch_write_device reads them in place
+    const long long n0 = d->n_in;
+    const size_t M = rational_outputs(n0, (long long)n, p.L, (long long)p.D1 * p.D2), J = rational_outputs(n0, (long long)n, 1, p.D1);
+    const size_t stride = pcm_row_stride(M);
     if (n > 0) {
         // a failed write leaves the output of the previous one described
         if (grow(&d->d_x, &d->x_cap, (size_t)(p.K1 - 1) + n, d->stream) || grow(&d->d_u, &d->u_cap, ((size_t)p.H2 + J) * p.cpad, d->stream) ||
@@ -2349,46 +2483,10 @@ int jaero_ddc_write_device(jaero_ddc *d, const void *d_iq, size_t n, int format)
     d->pcm_n = M; d->pcm_stride = stride;
     return JAERO_OK;
 }
-int jaero_ddc_write(jaero_ddc *d, const void *iq, size_t n, int format)
-{
-    if (!d || !iq) { set_error("jaero_ddc_write: null argument"); return JAERO_E_ARG; }
-    if (format != JAERO_IQ_CU8 && format != JAERO_IQ_CS16) { set_error("jaero_ddc_write: unknown IQ format"); return JAERO_E_ARG; }
-    if (n > ((size_t)1 << 34)) { set_error("jaero_ddc_write: too many samples in one write"); return JAERO_E_ARG; }
-    JB_CUDA(cudaSetDevice(d->device));
-    const size_t bytes = n * (format == JAERO_IQ_CU8 ? 2 : 4);
-    if (grow((uint8_t **)&d->d_raw, &d->raw_cap, std::max<size_t>(bytes, 4), d->stream)) return JAERO_E_CUDA;
-    if (bytes) {
-        JB_CUDA(cudaMemcpyAsync(d->d_raw, iq, bytes, cudaMemcpyHostToDevice, d->stream));
-        JB_CUDA(cudaStreamSynchronize(d->stream));                   // the caller may reuse its pageable buffer on return
-    }
-    return jaero_ddc_write_device(d, d->d_raw, n, format);
-}
-int jaero_ddc_output(jaero_ddc *d, const int16_t **d_pcm, size_t *n, size_t *stride)
-{
-    if (!d || !d_pcm || !n || !stride) { set_error("jaero_ddc_output: null argument"); return JAERO_E_ARG; }
-    *d_pcm = d->d_pcm; *n = d->pcm_n; *stride = d->pcm_stride;
-    return JAERO_OK;
-}
-int jaero_ddc_read_pcm(jaero_ddc *d, int16_t *out, size_t cap, size_t *n)
-{
-    if (!d || !out || !n) { set_error("jaero_ddc_read_pcm: null argument"); return JAERO_E_ARG; }
-    if (cap < d->pcm_n) { set_error("jaero_ddc_read_pcm: cap_per_channel is smaller than the last write's output"); return JAERO_E_ARG; }
-    JB_CUDA(cudaSetDevice(d->device));
-    if (d->pcm_n)
-        JB_CUDA(cudaMemcpy2DAsync(out, cap * sizeof(int16_t), d->d_pcm, d->pcm_stride * sizeof(int16_t), d->pcm_n * sizeof(int16_t),
-                                  d->p.n_channels, cudaMemcpyDeviceToHost, d->stream));
-    JB_CUDA(cudaStreamSynchronize(d->stream));
-    *n = d->pcm_n;
-    return JAERO_OK;
-}
-int jaero_ddc_set_stream(jaero_ddc *d, void *cuda_stream)
-{
-    if (!d) { set_error("null handle"); return JAERO_E_ARG; }
-    JB_CUDA(cudaSetDevice(d->device));
-    JB_CUDA(cudaStreamSynchronize(d->stream));
-    d->stream = cuda_stream ? (cudaStream_t)cuda_stream : d->own_stream;
-    return JAERO_OK;
-}
+int jaero_ddc_write(jaero_ddc *d, const void *iq, size_t n, int format) { return stage_iq_write(d, iq, n, format, "jaero_ddc_write", jaero_ddc_write_device); }
+int jaero_ddc_output(jaero_ddc *d, const int16_t **d_pcm, size_t *n, size_t *stride) { return pcm_output(d, d_pcm, n, stride, "jaero_ddc_output"); }
+int jaero_ddc_read_pcm(jaero_ddc *d, int16_t *out, size_t cap, size_t *n) { return pcm_read(d, out, cap, n, "jaero_ddc_read_pcm"); }
+int jaero_ddc_set_stream(jaero_ddc *d, void *cuda_stream) { return switch_stream(d, cuda_stream); }
 int jaero_ddc_set_offset(jaero_ddc *d, int channel, double hz)
 {
     if (!d || channel < -1 || channel >= d->p.n_channels) { set_error("jaero_ddc_set_offset: bad argument"); return JAERO_E_ARG; }
@@ -2407,17 +2505,7 @@ int jaero_ddc_set_audio_freq(jaero_ddc *d, int channel, double hz)
     for (int c = 0; c < d->p.n_channels; c++) if (channel < 0 || c == channel) d->S[c] = w;
     return ddc_upload_words(d, d->S, d->p.S, channel);
 }
-int jaero_ddc_get_stats(jaero_ddc *d, int64_t *inputs, int64_t *clipped)
-{
-    if (!d) { set_error("null handle"); return JAERO_E_ARG; }
-    if (inputs) *inputs = d->n_in;
-    if (clipped) {
-        JB_CUDA(cudaSetDevice(d->device));
-        JB_CUDA(cudaMemcpyAsync(clipped, d->p.clipped, d->p.n_channels * sizeof(int64_t), cudaMemcpyDeviceToHost, d->stream));
-        JB_CUDA(cudaStreamSynchronize(d->stream));
-    }
-    return JAERO_OK;
-}
+int jaero_ddc_get_stats(jaero_ddc *d, int64_t *inputs, int64_t *clipped) { return pcm_stats(d, inputs, clipped); }
 
 } // extern "C"
 
@@ -2459,14 +2547,10 @@ static void resample_design(const ResamplePlan &c, double *h)
     for (int k = 0; k < c.K; k++) h[k] *= c.L;
 }
 
-struct jaero_resample {
-    int device; cudaStream_t stream, own_stream;
-    std::vector<void *> allocs;
+struct jaero_resample : PcmStage {
     ResampleParams p;
-    long long n_in, launches;                                        // samples per channel written so far
     int16_t *d_in; size_t in_cap;                                    // host writes: the PCM staged on the device, [C][n]
     double *d_x; size_t x_cap;                                       // [H + n][cpad] rows of the current write
-    int16_t *d_pcm; size_t pcm_cap, pcm_n, pcm_stride;
 };
 
 extern "C" {
@@ -2497,9 +2581,9 @@ int jaero_resample_create(double input_rate, double output_rate, int n_channels,
     p.L = c.L; p.M = c.M; p.K = c.K;
     p.R = (c.K + c.L - 1) / c.L;
     p.H = p.R;                                                       // the first output of a write reads back R - 1 rows
-    std::vector<double> h(c.K), hp((size_t)c.L * p.R, 0.0);           // [L][R] per-phase taps, hp[phi][r] = h[phi + r L]
+    std::vector<double> h(c.K);
     resample_design(c, h.data());
-    for (int k = 0; k < c.K; k++) hp[(size_t)(k % c.L) * p.R + k / c.L] = h[k];
+    const std::vector<double> hp = polyphase_fold(h.data(), c.K, c.L, p.R);
     double *dhp;
     int rc = 0;
     rc |= owned_alloc(s, &dhp, hp.size());
@@ -2512,27 +2596,17 @@ int jaero_resample_create(double input_rate, double output_rate, int n_channels,
     *out = guard.release();
     return JAERO_OK;
 }
-void jaero_resample_destroy(jaero_resample *s)
-{
-    if (!s) return;
-    cudaSetDevice(s->device);
-    cudaStreamSynchronize(s->stream);
-    release(s, {s->d_in, s->d_x, s->d_pcm}, {}, s->own_stream);
-}
+void jaero_resample_destroy(jaero_resample *s) { if (s) destroy_stage(s, {s->d_in, s->d_x, s->d_pcm}); }
 int64_t jaero_resample_launch_count(const jaero_resample *s) { return s ? s->launches : 0; }
 
 int jaero_resample_write_device(jaero_resample *s, const int16_t *d_pcm, size_t n, size_t stride)
 {
-    if (!s || !d_pcm) { set_error("jaero_resample_write_device: null argument"); return JAERO_E_ARG; }
-    if ((uintptr_t)d_pcm & 1) { set_error("jaero_resample_write_device: PCM pointer not aligned to one sample"); return JAERO_E_ARG; }
-    if (stride < n) { set_error("jaero_resample_write_device: channel stride is smaller than n_samples"); return JAERO_E_ARG; }
-    if (n > ((size_t)1 << 34)) { set_error("jaero_resample_write_device: too many samples in one write"); return JAERO_E_ARG; }
+    int r = pcm_write_args(s, d_pcm, n, stride, true, "jaero_resample_write_device"); if (r) return r;
     JB_CUDA(cudaSetDevice(s->device));
     const ResampleParams &p = s->p;
     const long long n0 = s->n_in;
-    // outputs m with floor(m M / L) in [n0, n0 + n): ceil((n0 + n) L / M) - ceil(n0 L / M)
-    const size_t M_out = (size_t)(((n0 + (long long)n) * p.L + p.M - 1) / p.M - (n0 * p.L + p.M - 1) / p.M);
-    const size_t out_stride = std::max<size_t>(8, (M_out + 7) & ~(size_t)7);   // 16-byte rows: jaero_batch_write_device reads them in place
+    const size_t M_out = rational_outputs(n0, (long long)n, p.L, p.M);
+    const size_t out_stride = pcm_row_stride(M_out);
     if (n > 0) {
         // a failed write leaves the output of the previous one described
         if (grow(&s->d_x, &s->x_cap, ((size_t)p.H + n) * p.cpad, s->stream) ||
@@ -2545,78 +2619,33 @@ int jaero_resample_write_device(jaero_resample *s, const int16_t *d_pcm, size_t 
 }
 int jaero_resample_write(jaero_resample *s, const int16_t *pcm, size_t n, size_t stride)
 {
-    if (!s || !pcm) { set_error("jaero_resample_write: null argument"); return JAERO_E_ARG; }
-    if (stride < n) { set_error("jaero_resample_write: channel stride is smaller than n_samples"); return JAERO_E_ARG; }
-    if (n > ((size_t)1 << 34)) { set_error("jaero_resample_write: too many samples in one write"); return JAERO_E_ARG; }
-    JB_CUDA(cudaSetDevice(s->device));
-    const size_t C = (size_t)s->p.n_channels;
-    if (grow(&s->d_in, &s->in_cap, std::max<size_t>(C * n, 1), s->stream)) return JAERO_E_CUDA;
-    if (n) {
-        JB_CUDA(cudaMemcpy2DAsync(s->d_in, n * sizeof(int16_t), pcm, stride * sizeof(int16_t), n * sizeof(int16_t), C, cudaMemcpyHostToDevice,
-                                  s->stream));
-        JB_CUDA(cudaStreamSynchronize(s->stream));                   // the caller may reuse its pageable buffer on return
-    }
-    return jaero_resample_write_device(s, s->d_in, n, n);
+    return stage_pcm_write(s, pcm, n, stride, "jaero_resample_write", jaero_resample_write_device);
 }
 int jaero_resample_output(jaero_resample *s, const int16_t **d_pcm, size_t *n, size_t *stride)
 {
-    if (!s || !d_pcm || !n || !stride) { set_error("jaero_resample_output: null argument"); return JAERO_E_ARG; }
-    *d_pcm = s->d_pcm; *n = s->pcm_n; *stride = s->pcm_stride;
-    return JAERO_OK;
+    return pcm_output(s, d_pcm, n, stride, "jaero_resample_output");
 }
-int jaero_resample_read_pcm(jaero_resample *s, int16_t *out, size_t cap, size_t *n)
-{
-    if (!s || !out || !n) { set_error("jaero_resample_read_pcm: null argument"); return JAERO_E_ARG; }
-    if (cap < s->pcm_n) { set_error("jaero_resample_read_pcm: cap_per_channel is smaller than the last write's output"); return JAERO_E_ARG; }
-    JB_CUDA(cudaSetDevice(s->device));
-    if (s->pcm_n)
-        JB_CUDA(cudaMemcpy2DAsync(out, cap * sizeof(int16_t), s->d_pcm, s->pcm_stride * sizeof(int16_t), s->pcm_n * sizeof(int16_t),
-                                  s->p.n_channels, cudaMemcpyDeviceToHost, s->stream));
-    JB_CUDA(cudaStreamSynchronize(s->stream));
-    *n = s->pcm_n;
-    return JAERO_OK;
-}
-int jaero_resample_set_stream(jaero_resample *s, void *cuda_stream)
-{
-    if (!s) { set_error("null handle"); return JAERO_E_ARG; }
-    JB_CUDA(cudaSetDevice(s->device));
-    JB_CUDA(cudaStreamSynchronize(s->stream));
-    s->stream = cuda_stream ? (cudaStream_t)cuda_stream : s->own_stream;
-    return JAERO_OK;
-}
-int jaero_resample_get_stats(jaero_resample *s, int64_t *inputs, int64_t *clipped)
-{
-    if (!s) { set_error("null handle"); return JAERO_E_ARG; }
-    if (inputs) *inputs = s->n_in;
-    if (clipped) {
-        JB_CUDA(cudaSetDevice(s->device));
-        JB_CUDA(cudaMemcpyAsync(clipped, s->p.clipped, s->p.n_channels * sizeof(int64_t), cudaMemcpyDeviceToHost, s->stream));
-        JB_CUDA(cudaStreamSynchronize(s->stream));
-    }
-    return JAERO_OK;
-}
+int jaero_resample_read_pcm(jaero_resample *s, int16_t *out, size_t cap, size_t *n) { return pcm_read(s, out, cap, n, "jaero_resample_read_pcm"); }
+int jaero_resample_set_stream(jaero_resample *s, void *cuda_stream) { return switch_stream(s, cuda_stream); }
+int jaero_resample_get_stats(jaero_resample *s, int64_t *inputs, int64_t *clipped) { return pcm_stats(s, inputs, clipped); }
 
 } // extern "C"
 
 // ------------------------------------------------------------------ wideband carrier scanner
-struct jaero_scan {
-    int device; cudaStream_t stream, own_stream;
-    std::vector<void *> allocs;
+struct jaero_scan : Stage {
     ScanPlan p;
-    long long n_in, frames, launches;                                 // samples and complete frames since create / reset
+    long long frames;                                                // complete frames since create / reset (n_in: samples)
     double2 *d_carry;                                                // [nfft] samples frames * hop .. n_in - 1 (fewer than nfft)
     void *d_raw; size_t raw_cap;                                     // host writes: the IQ bytes staged on the device
     double2 *d_x, *d_work; double *d_pw; size_t x_cap, work_cap, pw_cap;
 };
-
-static bool pow2_nfft(int nfft) { return nfft >= 1024 && nfft <= 65536 && (nfft & (nfft - 1)) == 0; }
 
 extern "C" {
 
 int jaero_scan_create(double input_rate, int nfft, int hop, int device, jaero_scan **out)
 {
     if (!out) { set_error("jaero_scan_create: null argument"); return JAERO_E_ARG; }
-    if (!pow2_nfft(nfft)) { set_error("jaero_scan_create: nfft must be a power of two from 1024 to 65536"); return JAERO_E_ARG; }
+    if (!pow2_nfft(nfft, 65536)) { set_error("jaero_scan_create: nfft must be a power of two from 1024 to 65536"); return JAERO_E_ARG; }
     if (hop < 1 || hop > nfft) { set_error("jaero_scan_create: hop must be in [1, nfft]"); return JAERO_E_ARG; }
     if (!(input_rate > 0) || !std::isfinite(input_rate)) { set_error("jaero_scan_create: input_rate must be positive"); return JAERO_E_ARG; }
     CreateGuard<jaero_scan> guard(jaero_scan_destroy);
@@ -2625,88 +2654,42 @@ int jaero_scan_create(double input_rate, int nfft, int hop, int device, jaero_sc
     s->own_stream = s->stream;
     ScanPlan &p = s->p;
     p.nfft = nfft; p.hop = hop;
-    int lg = 0;
-    while ((1 << lg) < nfft) lg++;
-    p.n1 = 1 << (lg / 2); p.n2 = nfft / p.n1;
-    std::vector<double2> tw(nfft);
-    std::vector<double> win(nfft);
-    double wss = 0.0;
-    for (int k = 0; k < nfft; k++) {
-        const double a = 2 * M_PI * (double)k / nfft;
-        tw[k] = make_double2(cos(a), -sin(a));
-        win[k] = 0.5 - 0.5 * cos(a);
-        wss += win[k] * win[k];
-    }
-    p.inv_wss = 1.0 / wss;
-    double2 *dtw; double *dwin;
     int rc = 0;
-    rc |= owned_alloc(s, &dtw, (size_t)nfft); rc |= owned_alloc(s, &dwin, (size_t)nfft);
     rc |= owned_alloc(s, &p.sum, (size_t)nfft); rc |= owned_alloc(s, &p.maxh, (size_t)nfft);
     rc |= owned_alloc(s, &s->d_carry, (size_t)nfft);
     if (rc) return JAERO_E_CUDA;
-    p.tw = dtw; p.win = dwin;
-    JB_CUDA(cudaMemcpyAsync(dtw, tw.data(), nfft * sizeof(double2), cudaMemcpyHostToDevice, s->stream));
-    JB_CUDA(cudaMemcpyAsync(dwin, win.data(), nfft * sizeof(double), cudaMemcpyHostToDevice, s->stream));
-    JB_CUDA(cudaStreamSynchronize(s->stream));                       // the tables are in place, the host vectors may go
+    double wss;
+    if ((rc = four_step_tables(s, p, nfft, &wss))) return rc;
+    p.inv_wss = 1.0 / wss;
     *out = guard.release();
     return JAERO_OK;
 }
-void jaero_scan_destroy(jaero_scan *s)
-{
-    if (!s) return;
-    cudaSetDevice(s->device);
-    cudaStreamSynchronize(s->stream);
-    release(s, {s->d_raw, s->d_x, s->d_work, s->d_pw}, {}, s->own_stream);
-}
+void jaero_scan_destroy(jaero_scan *s) { if (s) destroy_stage(s, {s->d_raw, s->d_x, s->d_work, s->d_pw}); }
 int64_t jaero_scan_launch_count(const jaero_scan *s) { return s ? s->launches : 0; }
 
 int jaero_scan_write_device(jaero_scan *s, const void *d_iq, size_t n, int format)
 {
-    if (!s || !d_iq) { set_error("jaero_scan_write_device: null argument"); return JAERO_E_ARG; }
-    if (format != JAERO_IQ_CU8 && format != JAERO_IQ_CS16) { set_error("jaero_scan_write_device: unknown IQ format"); return JAERO_E_ARG; }
-    if ((uintptr_t)d_iq & (format == JAERO_IQ_CU8 ? 1 : 3)) { set_error("jaero_scan_write_device: IQ pointer not aligned to one sample"); return JAERO_E_ARG; }
-    if (n > ((size_t)1 << 34)) { set_error("jaero_scan_write_device: too many samples in one write"); return JAERO_E_ARG; }
+    int r = iq_write_args(s, d_iq, n, format, true, "jaero_scan_write_device"); if (r) return r;
     if (n == 0) return JAERO_OK;
     JB_CUDA(cudaSetDevice(s->device));
     const ScanPlan &p = s->p;
-    const long long N = p.nfft, hop = p.hop, total = s->n_in + (long long)n;
-    const long long x0 = s->frames * hop, carry = s->n_in - x0;      // xd[j] = sample x0 + j
-    const long long f_end = total >= N ? (total - N) / hop + 1 : 0, F = f_end - s->frames;
+    const long long N = p.nfft;
+    const FrameSpan w = frame_span(s->n_in, s->frames, N, p.hop, n);
     const int G = (int)std::max<long long>(1, SCAN_PASS_ELEMS / N);
-    const size_t g = (size_t)std::min<long long>(std::max<long long>(F, 1), G);
+    const size_t g = (size_t)std::min<long long>(std::max<long long>(w.F, 1), G);
     // every buffer is in place before anything is queued: a failed write leaves the average unchanged
-    if (grow(&s->d_x, &s->x_cap, (size_t)(carry + (long long)n), s->stream) || grow(&s->d_work, &s->work_cap, g * N, s->stream) ||
+    if (grow(&s->d_x, &s->x_cap, (size_t)(w.carry + (long long)n), s->stream) || grow(&s->d_work, &s->work_cap, g * N, s->stream) ||
         grow(&s->d_pw, &s->pw_cap, g * N, s->stream)) return JAERO_E_CUDA;
-    if (carry) JB_CUDA(cudaMemcpyAsync(s->d_x, s->d_carry, carry * sizeof(double2), cudaMemcpyDeviceToDevice, s->stream));
-    if (scan_convert(d_iq, format, (long long)n, s->d_x + carry, s->stream, &s->launches)) return JAERO_E_CUDA;
-    if (F > 0 && scan_frames(p, s->d_x, x0, s->frames, F, G, s->d_work, s->d_pw, s->stream, &s->launches)) return JAERO_E_CUDA;
-    const long long x1 = f_end * hop;                                // the first sample an incomplete frame needs
-    if (total > x1) JB_CUDA(cudaMemcpyAsync(s->d_carry, s->d_x + (x1 - x0), (total - x1) * sizeof(double2), cudaMemcpyDeviceToDevice, s->stream));
-    s->n_in = total; s->frames = f_end;
+    if (w.carry) JB_CUDA(cudaMemcpyAsync(s->d_x, s->d_carry, w.carry * sizeof(double2), cudaMemcpyDeviceToDevice, s->stream));
+    if (scan_convert(d_iq, format, (long long)n, s->d_x + w.carry, s->stream, &s->launches)) return JAERO_E_CUDA;
+    if (w.F > 0 && scan_frames(p, s->d_x, w.x0, s->frames, w.F, G, s->d_work, s->d_pw, s->stream, &s->launches)) return JAERO_E_CUDA;
+    if (w.total > w.x1)
+        JB_CUDA(cudaMemcpyAsync(s->d_carry, s->d_x + (w.x1 - w.x0), (w.total - w.x1) * sizeof(double2), cudaMemcpyDeviceToDevice, s->stream));
+    s->n_in = w.total; s->frames = w.f_end;
     return JAERO_OK;
 }
-int jaero_scan_write(jaero_scan *s, const void *iq, size_t n, int format)
-{
-    if (!s || !iq) { set_error("jaero_scan_write: null argument"); return JAERO_E_ARG; }
-    if (format != JAERO_IQ_CU8 && format != JAERO_IQ_CS16) { set_error("jaero_scan_write: unknown IQ format"); return JAERO_E_ARG; }
-    if (n > ((size_t)1 << 34)) { set_error("jaero_scan_write: too many samples in one write"); return JAERO_E_ARG; }
-    JB_CUDA(cudaSetDevice(s->device));
-    const size_t bytes = n * (format == JAERO_IQ_CU8 ? 2 : 4);
-    if (grow((uint8_t **)&s->d_raw, &s->raw_cap, std::max<size_t>(bytes, 4), s->stream)) return JAERO_E_CUDA;
-    if (bytes) {
-        JB_CUDA(cudaMemcpyAsync(s->d_raw, iq, bytes, cudaMemcpyHostToDevice, s->stream));
-        JB_CUDA(cudaStreamSynchronize(s->stream));                   // the caller may reuse its pageable buffer on return
-    }
-    return jaero_scan_write_device(s, s->d_raw, n, format);
-}
-int jaero_scan_set_stream(jaero_scan *s, void *cuda_stream)
-{
-    if (!s) { set_error("null handle"); return JAERO_E_ARG; }
-    JB_CUDA(cudaSetDevice(s->device));
-    JB_CUDA(cudaStreamSynchronize(s->stream));
-    s->stream = cuda_stream ? (cudaStream_t)cuda_stream : s->own_stream;
-    return JAERO_OK;
-}
+int jaero_scan_write(jaero_scan *s, const void *iq, size_t n, int format) { return stage_iq_write(s, iq, n, format, "jaero_scan_write", jaero_scan_write_device); }
+int jaero_scan_set_stream(jaero_scan *s, void *cuda_stream) { return switch_stream(s, cuda_stream); }
 int jaero_scan_reset(jaero_scan *s)
 {
     if (!s) { set_error("null handle"); return JAERO_E_ARG; }
@@ -2758,6 +2741,19 @@ static void scan_floor(const double *psd, int n, int W, double q, double *floor_
         floor_out[i] = psd[order[kth(k)]];
     }
 }
+// The floor of a spectrum of n bins over fs, once every bin is checked to be finite and >= 0: the q-quantile of a sliding window of
+// window_hz (odd, 3 to n bins)
+static int spectrum_floor(const double *psd, int n, double fs, double window_hz, double q, std::vector<double> &fl, const char *fn)
+{
+    for (int i = 0; i < n; i++)
+        if (!(psd[i] >= 0) || !std::isfinite(psd[i])) return arg_error(fn, "spectrum values must be finite and >= 0");
+    const double bin_hz = fs / n;
+    const double x = std::min(window_hz / bin_hz, (double)n);
+    const int W = std::min(std::max(2 * (int)std::floor(x / 2) + 1, 3), n);
+    fl.resize(n);
+    scan_floor(psd, n, W, q, fl.data());
+    return JAERO_OK;
+}
 
 // Nominal half-power widths of the continuous modes.
 //   OQPSK with root-raised-cosine pulses on each arm: the spectrum is a raised cosine of the symbol rate Rs = fb / 2, and a raised
@@ -2780,21 +2776,17 @@ extern "C" int jaero_scan_find_carriers(const double *psd, int nfft, double inpu
                                         jaero_carrier *out, int cap, int *n_found)
 {
     if (!psd || !n_found || (cap > 0 && !out) || cap < 0) { set_error("jaero_scan_find_carriers: bad argument"); return JAERO_E_ARG; }
-    if (!pow2_nfft(nfft)) { set_error("jaero_scan_find_carriers: nfft must be a power of two from 1024 to 65536"); return JAERO_E_ARG; }
+    if (!pow2_nfft(nfft, 65536)) { set_error("jaero_scan_find_carriers: nfft must be a power of two from 1024 to 65536"); return JAERO_E_ARG; }
     if (!(input_rate > 0) || !std::isfinite(input_rate)) { set_error("jaero_scan_find_carriers: input_rate must be positive"); return JAERO_E_ARG; }
     const jaero_scan_params P = params ? *params : jaero_scan_params{3.0, 100e3, 0.25, 200.0, 0.0};
     if (!(P.threshold_db > 0) || !std::isfinite(P.threshold_db) || !(P.floor_window_hz > 0) || !std::isfinite(P.floor_window_hz) ||
         !(P.floor_quantile >= 0 && P.floor_quantile <= 1) || !(P.min_width_hz >= 0) || !std::isfinite(P.min_width_hz) ||
         !(P.dc_guard_hz >= 0) || !std::isfinite(P.dc_guard_hz)) {
         set_error("jaero_scan_find_carriers: parameter out of range"); return JAERO_E_ARG; }
-    for (int i = 0; i < nfft; i++)
-        if (!(psd[i] >= 0) || !std::isfinite(psd[i])) { set_error("jaero_scan_find_carriers: spectrum values must be finite and >= 0"); return JAERO_E_ARG; }
     const int n = nfft;
+    std::vector<double> fl, e(n);
+    { const int r = spectrum_floor(psd, n, input_rate, P.floor_window_hz, P.floor_quantile, fl, "jaero_scan_find_carriers"); if (r) return r; }
     const double bin_hz = input_rate / n;
-    const double x = std::min(P.floor_window_hz / bin_hz, (double)n);
-    const int W = std::min(std::max(2 * (int)std::floor(x / 2) + 1, 3), n);
-    std::vector<double> fl(n), e(n);
-    scan_floor(psd, n, W, P.floor_quantile, fl.data());
     for (int i = 0; i < n; i++) e[i] = psd[i] - fl[i];
     const double thr = pow(10.0, P.threshold_db / 10.0);
     auto hz = [&](double i) { return (i - n / 2) * bin_hz; };
@@ -2847,18 +2839,15 @@ extern "C" int jaero_scan_find_carriers(const double *psd, int nfft, double inpu
 }
 
 // ------------------------------------------------------------------ mode identifier
-struct jaero_ident {
-    int device; cudaStream_t stream, own_stream;
-    std::vector<void *> allocs;
+struct jaero_ident : Stage {
     IdentPlan p;
-    long long n_in, frames, launches;                                 // samples and complete frames per channel since create / reset
+    long long frames;                                                // complete frames per channel since create / reset (n_in: samples)
     int16_t *d_carry;                                                // [C][nfft] samples frames * hop .. n_in - 1 (fewer than nfft)
     int16_t *d_in; size_t in_cap;                                    // host writes: the PCM staged on the device, [C][n]
     int16_t *d_x; size_t x_cap;                                      // [C][carry + n] the samples the write's frames read
     double2 *d_w0, *d_w1;                                            // [G][nfft] work matrices of one pass
 };
 
-static bool ident_nfft_ok(int nfft) { return nfft >= 1024 && nfft <= 16384 && (nfft & (nfft - 1)) == 0; }
 static bool ident_fs_ok(double fs) { return std::isfinite(fs) && fs >= 8000 && fs <= 192000 && fs == floor(fs); }
 static int ident_pass_frames(int nfft) { return (int)std::max<long long>(1, IDENT_PASS_ELEMS / nfft); }
 
@@ -2868,7 +2857,7 @@ int jaero_ident_create(double Fs, int n_channels, int nfft, int device, jaero_id
 {
     const char *fn = "jaero_ident_create";
     if (!out || n_channels <= 0) { set_error(std::string(fn) + ": bad argument"); return JAERO_E_ARG; }
-    if (!ident_nfft_ok(nfft)) { set_error(std::string(fn) + ": nfft must be a power of two from 1024 to 16384"); return JAERO_E_ARG; }
+    if (!pow2_nfft(nfft, 16384)) { set_error(std::string(fn) + ": nfft must be a power of two from 1024 to 16384"); return JAERO_E_ARG; }
     if (!ident_fs_ok(Fs)) { set_error(std::string(fn) + ": Fs must be whole hertz from 8000 to 192000"); return JAERO_E_ARG; }
     CreateGuard<jaero_ident> guard(jaero_ident_destroy);
     { const int e = guard.begin(fn, device); if (e) return e; }
@@ -2876,97 +2865,53 @@ int jaero_ident_create(double Fs, int n_channels, int nfft, int device, jaero_id
     d->own_stream = d->stream;
     IdentPlan &p = d->p;
     p.nfft = nfft; p.hop = nfft / 2; p.n_channels = n_channels;
-    int lg = 0;
-    while ((1 << lg) < nfft) lg++;
-    p.n1 = 1 << (lg / 2); p.n2 = nfft / p.n1;
-    std::vector<double2> tw(nfft);
-    std::vector<double> win(nfft);
-    double wss = 0.0;
-    for (int k = 0; k < nfft; k++) {
-        const double a = 2 * M_PI * (double)k / nfft;
-        tw[k] = make_double2(cos(a), -sin(a));
-        win[k] = 0.5 - 0.5 * cos(a);
-        wss += win[k] * win[k];
-    }
-    p.inv_wss2 = 1.0 / (wss * wss);
     const size_t work = (size_t)ident_pass_frames(nfft) * nfft;
-    double2 *dtw; double *dwin;
     int rc = 0;
-    rc |= owned_alloc(d, &dtw, (size_t)nfft); rc |= owned_alloc(d, &dwin, (size_t)nfft);
     rc |= owned_alloc(d, &p.sum, (size_t)n_channels * nfft);
     rc |= owned_alloc(d, &d->d_carry, (size_t)n_channels * nfft);
     rc |= owned_alloc(d, &d->d_w0, work); rc |= owned_alloc(d, &d->d_w1, work);
     if (rc) return JAERO_E_CUDA;
-    p.tw = dtw; p.win = dwin;
-    JB_CUDA(cudaMemcpyAsync(dtw, tw.data(), nfft * sizeof(double2), cudaMemcpyHostToDevice, d->stream));
-    JB_CUDA(cudaMemcpyAsync(dwin, win.data(), nfft * sizeof(double), cudaMemcpyHostToDevice, d->stream));
-    JB_CUDA(cudaStreamSynchronize(d->stream));                       // the tables are in place, the host vectors may go
+    double wss;
+    if ((rc = four_step_tables(d, p, nfft, &wss))) return rc;
+    p.inv_wss2 = 1.0 / (wss * wss);
     *out = guard.release();
     return JAERO_OK;
 }
-void jaero_ident_destroy(jaero_ident *d)
-{
-    if (!d) return;
-    cudaSetDevice(d->device);
-    cudaStreamSynchronize(d->stream);
-    release(d, {d->d_in, d->d_x}, {}, d->own_stream);
-}
+void jaero_ident_destroy(jaero_ident *d) { if (d) destroy_stage(d, {d->d_in, d->d_x}); }
 int64_t jaero_ident_launch_count(const jaero_ident *d) { return d ? d->launches : 0; }
 
 int jaero_ident_write_device(jaero_ident *d, const int16_t *d_pcm, size_t n, size_t stride)
 {
-    if (!d || !d_pcm) { set_error("jaero_ident_write_device: null argument"); return JAERO_E_ARG; }
-    if ((uintptr_t)d_pcm & 1) { set_error("jaero_ident_write_device: PCM pointer not aligned to one sample"); return JAERO_E_ARG; }
-    if (stride < n) { set_error("jaero_ident_write_device: channel stride is smaller than n_samples"); return JAERO_E_ARG; }
-    if (n > ((size_t)1 << 34)) { set_error("jaero_ident_write_device: too many samples in one write"); return JAERO_E_ARG; }
+    int r = pcm_write_args(d, d_pcm, n, stride, true, "jaero_ident_write_device"); if (r) return r;
     if (n == 0) return JAERO_OK;
     JB_CUDA(cudaSetDevice(d->device));
     const IdentPlan &p = d->p;
     const size_t C = (size_t)p.n_channels, B = sizeof(int16_t);
-    const long long N = p.nfft, hop = p.hop, total = d->n_in + (long long)n;
-    const long long x0 = d->frames * hop, carry = d->n_in - x0;      // d_x[c][j] = sample x0 + j of channel c
-    const long long f_end = total >= N ? (total - N) / hop + 1 : 0, F = f_end - d->frames;
-    if (F == 0) {                                                    // no frame completes: the samples join the carry
-        JB_CUDA(cudaMemcpy2DAsync(d->d_carry + carry, N * B, d_pcm, stride * B, n * B, C, cudaMemcpyDeviceToDevice, d->stream));
-        d->n_in = total;
+    const long long N = p.nfft;
+    const FrameSpan w = frame_span(d->n_in, d->frames, N, p.hop, n);  // d_x[c][j] = sample x0 + j of channel c
+    if (w.F == 0) {                                                  // no frame completes: the samples join the carry
+        JB_CUDA(cudaMemcpy2DAsync(d->d_carry + w.carry, N * B, d_pcm, stride * B, n * B, C, cudaMemcpyDeviceToDevice, d->stream));
+        d->n_in = w.total;
         return JAERO_OK;
     }
-    const size_t pitch = (size_t)(carry + (long long)n);
+    const size_t pitch = (size_t)(w.carry + (long long)n);
     // every buffer is in place before anything is queued: a failed write leaves the average unchanged
     if (grow(&d->d_x, &d->x_cap, C * pitch, d->stream)) return JAERO_E_CUDA;
-    if (carry) JB_CUDA(cudaMemcpy2DAsync(d->d_x, pitch * B, d->d_carry, N * B, carry * B, C, cudaMemcpyDeviceToDevice, d->stream));
-    JB_CUDA(cudaMemcpy2DAsync(d->d_x + carry, pitch * B, d_pcm, stride * B, n * B, C, cudaMemcpyDeviceToDevice, d->stream));
-    if (ident_frames(p, d->d_x, pitch, x0, d->frames, F, ident_pass_frames(p.nfft), d->d_w0, d->d_w1, d->stream, &d->launches))
+    if (w.carry) JB_CUDA(cudaMemcpy2DAsync(d->d_x, pitch * B, d->d_carry, N * B, w.carry * B, C, cudaMemcpyDeviceToDevice, d->stream));
+    JB_CUDA(cudaMemcpy2DAsync(d->d_x + w.carry, pitch * B, d_pcm, stride * B, n * B, C, cudaMemcpyDeviceToDevice, d->stream));
+    if (ident_frames(p, d->d_x, pitch, w.x0, d->frames, w.F, ident_pass_frames(p.nfft), d->d_w0, d->d_w1, d->stream, &d->launches))
         return JAERO_E_CUDA;
-    const long long x1 = f_end * hop;                                // the first sample an incomplete frame needs
-    if (total > x1)
-        JB_CUDA(cudaMemcpy2DAsync(d->d_carry, N * B, d->d_x + (x1 - x0), pitch * B, (total - x1) * B, C, cudaMemcpyDeviceToDevice, d->stream));
-    d->n_in = total; d->frames = f_end;
+    if (w.total > w.x1)
+        JB_CUDA(cudaMemcpy2DAsync(d->d_carry, N * B, d->d_x + (w.x1 - w.x0), pitch * B, (w.total - w.x1) * B, C, cudaMemcpyDeviceToDevice,
+                                  d->stream));
+    d->n_in = w.total; d->frames = w.f_end;
     return JAERO_OK;
 }
 int jaero_ident_write(jaero_ident *d, const int16_t *pcm, size_t n, size_t stride)
 {
-    if (!d || !pcm) { set_error("jaero_ident_write: null argument"); return JAERO_E_ARG; }
-    if (stride < n) { set_error("jaero_ident_write: channel stride is smaller than n_samples"); return JAERO_E_ARG; }
-    if (n > ((size_t)1 << 34)) { set_error("jaero_ident_write: too many samples in one write"); return JAERO_E_ARG; }
-    JB_CUDA(cudaSetDevice(d->device));
-    const size_t C = (size_t)d->p.n_channels;
-    if (grow(&d->d_in, &d->in_cap, std::max<size_t>(C * n, 1), d->stream)) return JAERO_E_CUDA;
-    if (n) {
-        JB_CUDA(cudaMemcpy2DAsync(d->d_in, n * sizeof(int16_t), pcm, stride * sizeof(int16_t), n * sizeof(int16_t), C, cudaMemcpyHostToDevice,
-                                  d->stream));
-        JB_CUDA(cudaStreamSynchronize(d->stream));                   // the caller may reuse its pageable buffer on return
-    }
-    return jaero_ident_write_device(d, d->d_in, n, n);
+    return stage_pcm_write(d, pcm, n, stride, "jaero_ident_write", jaero_ident_write_device);
 }
-int jaero_ident_set_stream(jaero_ident *d, void *cuda_stream)
-{
-    if (!d) { set_error("null handle"); return JAERO_E_ARG; }
-    JB_CUDA(cudaSetDevice(d->device));
-    JB_CUDA(cudaStreamSynchronize(d->stream));
-    d->stream = cuda_stream ? (cudaStream_t)cuda_stream : d->own_stream;
-    return JAERO_OK;
-}
+int jaero_ident_set_stream(jaero_ident *d, void *cuda_stream) { return switch_stream(d, cuda_stream); }
 int jaero_ident_reset(jaero_ident *d)
 {
     if (!d) { set_error("null handle"); return JAERO_E_ARG; }
@@ -2993,19 +2938,15 @@ int jaero_ident_classify(const double *sq_mean, int nfft, double Fs, const jaero
 {
     const char *fn = "jaero_ident_classify";
     if (!sq_mean || !out) { set_error(std::string(fn) + ": null argument"); return JAERO_E_ARG; }
-    if (!ident_nfft_ok(nfft)) { set_error(std::string(fn) + ": nfft must be a power of two from 1024 to 16384"); return JAERO_E_ARG; }
+    if (!pow2_nfft(nfft, 16384)) { set_error(std::string(fn) + ": nfft must be a power of two from 1024 to 16384"); return JAERO_E_ARG; }
     if (!ident_fs_ok(Fs)) { set_error(std::string(fn) + ": Fs must be whole hertz from 8000 to 192000"); return JAERO_E_ARG; }
     const jaero_ident_params P = params ? *params : jaero_ident_params{5.0, 400.0, 0.5};
     if (!std::isfinite(P.threshold_db) || !(P.floor_window_hz > 0) || !std::isfinite(P.floor_window_hz) ||
         !(P.floor_quantile >= 0 && P.floor_quantile <= 1)) { set_error(std::string(fn) + ": parameter out of range"); return JAERO_E_ARG; }
     const int n = nfft;
-    for (int i = 0; i < n; i++)
-        if (!(sq_mean[i] >= 0) || !std::isfinite(sq_mean[i])) { set_error(std::string(fn) + ": spectrum values must be finite and >= 0"); return JAERO_E_ARG; }
+    std::vector<double> fl, Q(n);
+    { const int e = spectrum_floor(sq_mean, n, Fs, P.floor_window_hz, P.floor_quantile, fl, fn); if (e) return e; }
     const double bin_hz = Fs / n;
-    const double x = std::min(P.floor_window_hz / bin_hz, (double)n);
-    const int W = std::min(std::max(2 * (int)std::floor(x / 2) + 1, 3), n);
-    std::vector<double> fl(n), Q(n);
-    scan_floor(sq_mean, n, W, P.floor_quantile, fl.data());
     for (int i = 0; i < n; i++) Q[i] = fl[i] > 0 ? sq_mean[i] / fl[i] : 0.0;
     static const double fbs[4] = {600.0, 1200.0, 8400.0, 10500.0};
     static const int modes[4] = {JAERO_MODE_MSK600, JAERO_MODE_MSK1200, JAERO_MODE_OQPSK8400, JAERO_MODE_OQPSK10500};

@@ -1,7 +1,7 @@
 // Double-precision complex arithmetic and FFT building blocks: the complex helpers and butterflies of every device FFT (coarse
 // estimator, wideband scanner, FFT convolution, trident FFTs) and the demodulators' complex products, plus the Stockham autosort
 // pass with radix-8 / radix-4 butterflies kept in registers over TILE independent sequences held in natural order in shared
-// memory rows s[f][.] (row pitch LD) that the estimator and the scanner use.
+// memory rows s[f][.] (row pitch LD) that the estimator, the scanner and the identifier use.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -80,6 +80,59 @@ __device__ __forceinline__ void stockham_pass(double2 (*s)[LD], int n, int Ns, c
             }
         }
         __syncthreads();
+    }
+}
+
+// The tile steps of the four-step FFTs of the wideband scanner and the mode identifier: TILE rows of up to MAXN points in
+// s[f][.] (row pitch MAXN + 1), THREADS threads, an N = n1 x n2 point transform whose x[n2 r + c] is the tile's column c, row r.
+
+// TILE transforms of length n in {32, 64, 128}, and 256 when MAXN allows it: 256 = 8*8*4, 128 = 8*4*4, 64 = 8*8, 32 = 8*4.
+// Unscaled in both directions.
+template <bool INV, int TILE, int MAXN, int THREADS>
+__device__ __forceinline__ void tile_fft(double2 (*s)[MAXN + 1], int n, const double2 *__restrict__ tw, int tw_stride)
+{
+    stockham_pass<INV, 8, TILE, MAXN + 1, THREADS>(s, n, 1, tw, tw_stride);
+    if (MAXN >= 256 && n == 256) {
+        stockham_pass<INV, 8, TILE, MAXN + 1, THREADS>(s, n, 8, tw, tw_stride);
+        stockham_pass<INV, 4, TILE, MAXN + 1, THREADS>(s, n, 64, tw, tw_stride);
+    } else if (n == 128) {
+        stockham_pass<INV, 4, TILE, MAXN + 1, THREADS>(s, n, 8, tw, tw_stride);
+        stockham_pass<INV, 4, TILE, MAXN + 1, THREADS>(s, n, 32, tw, tw_stride);
+    } else if (n == 64) stockham_pass<INV, 8, TILE, MAXN + 1, THREADS>(s, n, 8, tw, tw_stride);
+    else stockham_pass<INV, 4, TILE, MAXN + 1, THREADS>(s, n, 8, tw, tw_stride);
+}
+
+// Column tile out, after the n1-point FFTs: out[k1 n2 + c] = s[c - c0][k1] W_N^(c k1)
+template <int TILE, int LD, int THREADS>
+__device__ __forceinline__ void store_cols_twiddled(double2 (*s)[LD], int n1, int n2, int N, int c0, const double2 *__restrict__ tw,
+                                                    double2 *__restrict__ out)
+{
+    for (int e = threadIdx.x; e < n1 * TILE; e += THREADS) {
+        const int k1 = e / TILE, cc = e - k1 * TILE;
+        const int c = c0 + cc;
+        out[(size_t)k1 * n2 + c] = c_mul(s[cc][k1], __ldg(tw + ((c * k1) & (N - 1))));
+    }
+}
+
+// Row tile in: s[rr][c] = in[(r0 + rr) n2 + c]
+template <int TILE, int LD, int THREADS>
+__device__ __forceinline__ void load_rows(double2 (*s)[LD], int n2, int r0, const double2 *__restrict__ in)
+{
+    for (int e = threadIdx.x; e < n2 * TILE; e += THREADS) {
+        const int rr = e / n2, c = e - rr * n2;
+        s[rr][c] = in[(size_t)(r0 + rr) * n2 + c];
+    }
+}
+
+// Row tile out, after the n2-point FFTs: X[k1 + n1 k2] sits at s[k1 - r0][k2]; |X|^2 scale goes to its fftshift index
+// i = (k + N/2) mod N = k1 + n1 ((k2 + n2/2) mod n2)
+template <int TILE, int LD, int THREADS>
+__device__ __forceinline__ void store_power_shifted(double2 (*s)[LD], int n1, int n2, int r0, double scale, double *__restrict__ out)
+{
+    for (int e = threadIdx.x; e < n2 * TILE; e += THREADS) {
+        const int k2 = e / TILE, rr = e - k2 * TILE;                 // rr fastest: TILE consecutive bins per k2
+        const double2 v = s[rr][k2];
+        out[(r0 + rr) + n1 * ((k2 + (n2 >> 1)) & (n2 - 1))] = (v.x * v.x + v.y * v.y) * scale;
     }
 }
 

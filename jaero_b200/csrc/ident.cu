@@ -24,30 +24,14 @@ namespace jb {
 
 typedef double2 IdentRow[IDENT_MAXN + 1];
 
-template <bool INV, int R>
-__device__ __forceinline__ void ident_pass(IdentRow *s, int n, int Ns, const double2 *__restrict__ tw, int tw_stride)
-{
-    stockham_pass<INV, R, IDENT_TILE, IDENT_MAXN + 1, IDENT_THREADS>(s, n, Ns, tw, tw_stride);
-}
-
-// IDENT_TILE transforms of length n in {32, 64, 128}: 128 = 8*4*4, 64 = 8*8, 32 = 8*4. Unscaled in both directions.
 template <bool INV>
 __device__ __forceinline__ void ident_tile_fft(IdentRow *s, int n, const double2 *__restrict__ tw, int tw_stride)
 {
-    ident_pass<INV, 8>(s, n, 1, tw, tw_stride);
-    if (n == 128) { ident_pass<INV, 4>(s, n, 8, tw, tw_stride); ident_pass<INV, 4>(s, n, 32, tw, tw_stride); }
-    else if (n == 64) ident_pass<INV, 8>(s, n, 8, tw, tw_stride);
-    else ident_pass<INV, 4>(s, n, 8, tw, tw_stride);
+    tile_fft<INV, IDENT_TILE, IDENT_MAXN, IDENT_THREADS>(s, n, tw, tw_stride);
 }
-
-// Column tile out: out[k1 n2 + c] = s[c - c0][k1] W_N^(c k1)
 __device__ __forceinline__ void ident_store_cols(const IdentPlan &p, IdentRow *s, int c0, double2 *__restrict__ out)
 {
-    for (int e = threadIdx.x; e < p.n1 * IDENT_TILE; e += IDENT_THREADS) {
-        const int k1 = e / IDENT_TILE, cc = e - k1 * IDENT_TILE;
-        const int c = c0 + cc;
-        out[(size_t)k1 * p.n2 + c] = c_mul(s[cc][k1], __ldg(p.tw + ((c * k1) & (p.nfft - 1))));
-    }
+    store_cols_twiddled<IDENT_TILE, IDENT_MAXN + 1, IDENT_THREADS>(s, p.n1, p.n2, p.nfft, c0, p.tw, out);
 }
 
 // grid (n2 / IDENT_TILE, frames of the pass); pass item j0 + blockIdx.y is frame f0 + (j mod F) of channel j / F
@@ -77,11 +61,7 @@ __global__ void __launch_bounds__(IDENT_THREADS) ident_mask_kernel(IdentPlan p, 
     IdentRow *s = reinterpret_cast<IdentRow *>(ident_smem);
     const int n1 = p.n1, n2 = p.n2, N = p.nfft;
     const int r0 = blockIdx.x * IDENT_TILE;
-    const double2 *in = w0 + (size_t)blockIdx.y * N;
-    for (int e = threadIdx.x; e < n2 * IDENT_TILE; e += IDENT_THREADS) {
-        const int rr = e / n2, c = e - rr * n2;
-        s[rr][c] = in[(size_t)(r0 + rr) * n2 + c];
-    }
+    load_rows<IDENT_TILE, IDENT_MAXN + 1, IDENT_THREADS>(s, n2, r0, w0 + (size_t)blockIdx.y * N);
     __syncthreads();
     ident_tile_fft<false>(s, n2, p.tw, N / n2);
     // X[k1 + n1 k2] sits at s[k1 - r0][k2]. 2/N is a power of two, so folding the inverse's 1/N in here rounds nothing.
@@ -135,20 +115,10 @@ __global__ void __launch_bounds__(IDENT_THREADS) ident_power_kernel(IdentPlan p,
     IdentRow *s = reinterpret_cast<IdentRow *>(ident_smem);
     const int n1 = p.n1, n2 = p.n2, N = p.nfft;
     const int r0 = blockIdx.x * IDENT_TILE;
-    const double2 *in = w0 + (size_t)blockIdx.y * N;
-    for (int e = threadIdx.x; e < n2 * IDENT_TILE; e += IDENT_THREADS) {
-        const int rr = e / n2, c = e - rr * n2;
-        s[rr][c] = in[(size_t)(r0 + rr) * n2 + c];
-    }
+    load_rows<IDENT_TILE, IDENT_MAXN + 1, IDENT_THREADS>(s, n2, r0, w0 + (size_t)blockIdx.y * N);
     __syncthreads();
     ident_tile_fft<false>(s, n2, p.tw, N / n2);
-    // fftshift: i = (k + N/2) mod N = k1 + n1 ((k2 + n2/2) mod n2)
-    double *out = pw + (size_t)blockIdx.y * N;
-    for (int e = threadIdx.x; e < n2 * IDENT_TILE; e += IDENT_THREADS) {
-        const int k2 = e / IDENT_TILE, rr = e - k2 * IDENT_TILE;      // rr fastest: 16 consecutive bins per k2
-        const double2 v = s[rr][k2];
-        out[(r0 + rr) + n1 * ((k2 + (n2 >> 1)) & (n2 - 1))] = (v.x * v.x + v.y * v.y) * p.inv_wss2;
-    }
+    store_power_shifted<IDENT_TILE, IDENT_MAXN + 1, IDENT_THREADS>(s, n1, n2, r0, p.inv_wss2, pw + (size_t)blockIdx.y * N);
 }
 
 // grid (nfft / 256, channels the pass touches); pw row g is pass item j0 + g

@@ -18,20 +18,9 @@ namespace jb {
 
 typedef double2 ScanRow[SCAN_MAXN + 1];
 
-template <int R>
-__device__ __forceinline__ void scan_pass(ScanRow *s, int n, int Ns, const double2 *__restrict__ tw, int tw_stride)
-{
-    stockham_pass<false, R, SCAN_TILE, SCAN_MAXN + 1, SCAN_THREADS>(s, n, Ns, tw, tw_stride);
-}
-
-// SCAN_TILE forward FFTs of length n in {32, 64, 128, 256}: 256 = 8*8*4, 128 = 8*4*4, 64 = 8*8, 32 = 8*4
 __device__ __forceinline__ void scan_tile_fft(ScanRow *s, int n, const double2 *__restrict__ tw, int tw_stride)
 {
-    scan_pass<8>(s, n, 1, tw, tw_stride);
-    if (n == 256) { scan_pass<8>(s, n, 8, tw, tw_stride); scan_pass<4>(s, n, 64, tw, tw_stride); }
-    else if (n == 128) { scan_pass<4>(s, n, 8, tw, tw_stride); scan_pass<4>(s, n, 32, tw, tw_stride); }
-    else if (n == 64) scan_pass<8>(s, n, 8, tw, tw_stride);
-    else scan_pass<4>(s, n, 8, tw, tw_stride);
+    tile_fft<false, SCAN_TILE, SCAN_MAXN, SCAN_THREADS>(s, n, tw, tw_stride);
 }
 
 __global__ void scan_convert_kernel(const void *raw, int format, long long n, double2 *xd)
@@ -58,12 +47,7 @@ __global__ void __launch_bounds__(SCAN_THREADS) scan_col_kernel(ScanPlan p, cons
     }
     __syncthreads();
     scan_tile_fft(s, n1, p.tw, N / n1);
-    double2 *out = work + (size_t)blockIdx.y * N;
-    for (int e = threadIdx.x; e < n1 * SCAN_TILE; e += SCAN_THREADS) {
-        const int k1 = e / SCAN_TILE, cc = e - k1 * SCAN_TILE;
-        const int c = c0 + cc;
-        out[(size_t)k1 * n2 + c] = c_mul(s[cc][k1], __ldg(p.tw + ((c * k1) & (N - 1))));
-    }
+    store_cols_twiddled<SCAN_TILE, SCAN_MAXN + 1, SCAN_THREADS>(s, n1, n2, N, c0, p.tw, work + (size_t)blockIdx.y * N);
 }
 
 // grid (n1 / SCAN_TILE, frames of the pass)
@@ -73,20 +57,10 @@ __global__ void __launch_bounds__(SCAN_THREADS) scan_row_kernel(ScanPlan p, cons
     ScanRow *s = reinterpret_cast<ScanRow *>(scan_smem);
     const int n1 = p.n1, n2 = p.n2, N = p.nfft;
     const int r0 = blockIdx.x * SCAN_TILE;
-    const double2 *in = work + (size_t)blockIdx.y * N;
-    for (int e = threadIdx.x; e < n2 * SCAN_TILE; e += SCAN_THREADS) {
-        const int rr = e / n2, c = e - rr * n2;
-        s[rr][c] = in[(size_t)(r0 + rr) * n2 + c];
-    }
+    load_rows<SCAN_TILE, SCAN_MAXN + 1, SCAN_THREADS>(s, n2, r0, work + (size_t)blockIdx.y * N);
     __syncthreads();
     scan_tile_fft(s, n2, p.tw, N / n2);
-    // X[k1 + n1 k2] sits at s[k1 - r0][k2]; fftshift: i = (k + N/2) mod N = k1 + n1 ((k2 + n2/2) mod n2)
-    double *out = pw + (size_t)blockIdx.y * N;
-    for (int e = threadIdx.x; e < n2 * SCAN_TILE; e += SCAN_THREADS) {
-        const int k2 = e / SCAN_TILE, rr = e - k2 * SCAN_TILE;        // rr fastest: 16 consecutive bins per k2
-        const double2 v = s[rr][k2];
-        out[(r0 + rr) + n1 * ((k2 + (n2 >> 1)) & (n2 - 1))] = (v.x * v.x + v.y * v.y) * p.inv_wss;
-    }
+    store_power_shifted<SCAN_TILE, SCAN_MAXN + 1, SCAN_THREADS>(s, n1, n2, r0, p.inv_wss, pw + (size_t)blockIdx.y * N);
 }
 
 __global__ void scan_accumulate_kernel(ScanPlan p, const double *__restrict__ pw, int F)
