@@ -1203,3 +1203,6 @@ def probe_carriers(carriers, input_rate, iq, fmt, interpolation=1, decimation=No
             d["mode"] = "unknown"
         out.append(d)
     return out
+
+
+from .receiver import Receiver  # noqa: E402  (built on the classes above)

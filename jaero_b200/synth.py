@@ -135,6 +135,52 @@ def _pchannel_bits_once(fp, rng, n_frames, uw_bits, n_sus, scr, loop, even_parit
     return allbits, np.stack(all_sus)
 
 
+FILL_SU = bytes([0x01] + [0] * 9)       # the payload pchannel_bits_from_sus pads the last frame with (the Reassembler skips type 0x01)
+
+
+def pchannel_bits_from_sus(fb, sus, loop=False, even_parity=False):
+    """Serial channel bits of P-channel frames carrying the given signal units, in order (a transmitter for known messages).
+
+    sus: a sequence of 10-byte payloads (the CRC-16 is appended) or 12-byte signal units (sent as they are). The last frame is
+    padded with FILL_SU. loop and even_parity as in pchannel_bits. The frames are laid out as pchannel_bits lays them out; the
+    10.5 kbps header's dummy bits come from a fixed seed, so equal arguments give equal bits."""
+    fp = frame_params(fb)
+    n_sus = fp["blocks"] * 64 * fp["cols"] // 2 // 96
+    units = []
+    for su in list(sus):
+        b = np.frombuffer(bytes(bytearray(su)), dtype=np.uint8)
+        if len(b) == 10:
+            c = crc16(b)
+            b = np.concatenate([b, np.array([c & 0xFF, c >> 8], dtype=np.uint8)])
+        if len(b) != 12:
+            raise ValueError("a signal unit has 10 payload bytes or 12 bytes with its CRC, got %d" % len(b))
+        units.append(b)
+    fill = np.frombuffer(FILL_SU, dtype=np.uint8)
+    c = crc16(fill)
+    fill = np.concatenate([fill, np.array([c & 0xFF, c >> 8], dtype=np.uint8)])
+    units += [fill] * ((-len(units)) % n_sus if units else n_sus)
+    n_frames = len(units) // n_sus
+    uw_bits = np.array([(UW >> (31 - i)) & 1 for i in range(32)], dtype=np.uint8)
+    scr = scrambler_sequence(n_sus * 96)
+    payloads = [np.unpackbits(np.concatenate(units[f * n_sus:(f + 1) * n_sus]), bitorder="little") ^ scr for f in range(n_frames)]
+    dummies = np.random.default_rng(0).integers(0, 2, size=(n_frames, fp["header_extra"]), dtype=np.uint8)
+    enc_state = 0
+    if loop:                                                      # tail-biting: start in the state the last frame ends in
+        for b in payloads[-1][-7:]:
+            enc_state = ((enc_state << 1) | int(b)) & 127
+    uw = np.repeat(uw_bits, 2) if fp["uw_interleaved"] else uw_bits
+    frames = []
+    for f in range(n_frames):
+        coded, enc_state = conv_encode_stream(payloads[f], enc_state)
+        blocks = [interleave(coded[b * 64 * fp["cols"]:(b + 1) * 64 * fp["cols"]], fp["cols"]) for b in range(fp["blocks"])]
+        header = np.array([(0x1000 | ((f & 15) << 4) | (f & 15)) >> (15 - i) & 1 for i in range(16)], dtype=np.uint8)
+        frames.append(np.concatenate([uw, header, dummies[f]] + blocks))
+    allbits = np.concatenate(frames)
+    if even_parity and (int(allbits.sum()) & 1):
+        allbits[(n_frames - 1) * fp["frame_bits"] + len(uw) + 7] ^= 1     # last frame's super-frame marker, as pchannel_bits
+    return allbits
+
+
 def rrc_pulse(alpha, span_symbols, sps):
     """Root-raised-cosine pulse sampled at `sps` samples/symbol (closed form as DSP.h:316-338)."""
     n = int(round(span_symbols * sps))
