@@ -793,6 +793,13 @@ class CChannelBatch(_Handle):
             res.append((su[:, :, :12].copy(), su[:, :, 12].astype(np.int32), r[:, 48:348].copy(), r[:, 348:352].copy().view(np.int32).reshape(-1)))
         return res
 
+    def read_frames_raw(self, out, counts):
+        """The C-ABI call without per-channel Python objects, into out[n_channels, cap, RECORD] uint8 and counts[n_channels]
+        int32; record = 3 x (12 SU bytes, crc_ok, 3 pad), 300 voice bytes, frame number (int32). -> (out, counts)"""
+        assert out.dtype == np.uint8 and out.shape[0] == self.n and out.shape[2] == self.RECORD and out.flags.c_contiguous
+        _check(lib().jaero_cchannel_read_frames(self.h, _p(out), out.shape[1], _p(counts)))
+        return out, counts
+
     def stats(self):
         dcd = np.zeros(self.n, dtype=np.int32); tot = np.zeros(self.n, dtype=np.int64); ok = np.zeros(self.n, dtype=np.int64)
         _check(lib().jaero_cchannel_get_stats(self.h, _p(dcd), _p(tot), _p(ok)))
@@ -1206,3 +1213,4 @@ def probe_carriers(carriers, input_rate, iq, fmt, interpolation=1, decimation=No
 
 
 from .receiver import Receiver  # noqa: E402  (built on the classes above)
+from .recording import RecordingDecoder  # noqa: E402

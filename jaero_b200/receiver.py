@@ -190,7 +190,7 @@ class Receiver:
                                 device=self.device)
         plans, self._unplanned = channel_plan(probed, self.input_rate, self.decimation, self.interpolation)
         for mode in sorted(plans, key=lambda m: plans[m]["carriers"][0]["center_hz"]):
-            g = _Group(mode, plans[mode], len(self._carriers), self.device, self.stream)
+            g = self._new_group(mode, plans[mode], len(self._carriers))
             self._groups.append(g)
             for c in plans[mode]["carriers"]:
                 self._carriers.append(dict(c, mode=mode))
@@ -202,6 +202,9 @@ class Receiver:
         ev = self._feed(acq.data_ptr(), n)                            # the acquisition window, decoded like any other IQ
         del acq                                                        # freed in stream order: the blocks above come first
         return ev
+
+    def _new_group(self, mode, plan, first):
+        return _Group(mode, plan, first, self.device, self.stream)
 
     # ---------------------------------------------------------------------------------------------------------- blocks
     def _block(self, ptr, n):
@@ -220,38 +223,47 @@ class Receiver:
         self._ticks += due
         return self._read()
 
-    def _event(self, kind, c, **fields):
+    def _event(self, kind, c, t, **fields):
         car = self._carriers[c]
-        return dict(kind=kind, carrier=c, center_hz=car["center_hz"], mode=car["mode"], input_seconds=self._n_in / self.input_rate,
-                    **fields)
+        return dict(kind=kind, carrier=c, center_hz=car["center_hz"], mode=car["mode"], input_seconds=t, **fields)
 
     def _read(self):
-        ev = []
+        ev, t = [], self._n_in / self.input_rate
         for g in self._groups:
             if g.mode in P_MODES:
                 out, counts = g.layer.read_sus_raw(g.su_out, g.su_counts)
                 for ch in np.flatnonzero(counts):
-                    c = g.first + int(ch)
-                    recs = out[ch, :counts[ch]]
-                    ok = recs[:, 12] != 0
-                    self._su_total[c] += len(recs); self._su_bad[c] += int((~ok).sum())
-                    rs = self._reasm[c]
-                    for r in recs[ok]:
-                        su = r[:12].tobytes()
-                        if self.emit_sus:
-                            ev.append(self._event("su", c, su=su, index=int(r[13]), frame=int(r[14]) | (int(r[15]) << 8)))
-                        rs.push_su(su)
-                    for rec in rs.pop_all():
-                        rec["record_kind"], rec["acars_mode"] = rec.pop("kind"), rec.pop("mode")
-                        self._messages[c] += 1
-                        ev.append(self._event("acars", c, **rec))
+                    ev += self._units(g.first + int(ch), out[ch, :counts[ch]], t)
             else:
                 for ch, (su, ok, voice, frame) in enumerate(g.layer.read_frames()):
-                    c = g.first + ch
-                    for k in range(len(frame)):
-                        self._frames[c] += 1; self._su_total[c] += 3; self._su_bad[c] += int((ok[k] == 0).sum())
-                        ev.append(self._event("cframe", c, sus=[x.tobytes() for x in su[k]], crc_ok=[bool(x) for x in ok[k]],
-                                              voice=voice[k].tobytes(), frame=int(frame[k])))
+                    ev += self._cframes(g.first + ch, su, ok, voice, frame, t)
+        return ev
+
+    def _units(self, c, recs, t):
+        """carrier c's signal-unit records (read_sus_raw rows), decoded by input second t: counted, the CRC-valid ones pushed to
+        the carrier's Reassembler -> their "su" (with emit_sus) and "acars" events"""
+        ev = []
+        ok = recs[:, 12] != 0
+        self._su_total[c] += len(recs); self._su_bad[c] += int((~ok).sum())
+        rs = self._reasm[c]
+        for r in recs[ok]:
+            su = r[:12].tobytes()
+            if self.emit_sus:
+                ev.append(self._event("su", c, t, su=su, index=int(r[13]), frame=int(r[14]) | (int(r[15]) << 8)))
+            rs.push_su(su)
+        for rec in rs.pop_all():
+            rec["record_kind"], rec["acars_mode"] = rec.pop("kind"), rec.pop("mode")
+            self._messages[c] += 1
+            ev.append(self._event("acars", c, t, **rec))
+        return ev
+
+    def _cframes(self, c, su, ok, voice, frame, t):
+        """carrier c's C-channel frames (read_frames arrays), decoded by input second t: counted -> their "cframe" events"""
+        ev = []
+        for k in range(len(frame)):
+            self._frames[c] += 1; self._su_total[c] += 3; self._su_bad[c] += int((ok[k] == 0).sum())
+            ev.append(self._event("cframe", c, t, sus=[x.tobytes() for x in su[k]], crc_ok=[bool(x) for x in ok[k]],
+                                  voice=voice[k].tobytes(), frame=int(frame[k])))
         return ev
 
     # ---------------------------------------------------------------------------------------------------------- state
