@@ -1214,3 +1214,4 @@ def probe_carriers(carriers, input_rate, iq, fmt, interpolation=1, decimation=No
 
 from .receiver import Receiver  # noqa: E402  (built on the classes above)
 from .recording import RecordingDecoder  # noqa: E402
+from .audio import AudioDecoder  # noqa: E402

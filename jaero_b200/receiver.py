@@ -43,7 +43,44 @@ class _Group:
                 o.close()
 
 
-class Receiver:
+class _Events:
+    """Event formation shared by the decoders: a carrier's signal-unit records or C-channel frames -> its events, counted per
+    carrier. Needs self._carriers (carrier index -> dict with mode and center_hz), self._reasm (its Reassembler, P-channel
+    carriers), self.emit_sus and the counters self._su_total, self._su_bad, self._messages and self._frames."""
+
+    def _event(self, kind, c, t, **fields):
+        car = self._carriers[c]
+        return dict(kind=kind, carrier=c, center_hz=car["center_hz"], mode=car["mode"], input_seconds=t, **fields)
+
+    def _units(self, c, recs, t):
+        """carrier c's signal-unit records (read_sus_raw rows), decoded by input second t: counted, the CRC-valid ones pushed to
+        the carrier's Reassembler -> their "su" (with emit_sus) and "acars" events"""
+        ev = []
+        ok = recs[:, 12] != 0
+        self._su_total[c] += len(recs); self._su_bad[c] += int((~ok).sum())
+        rs = self._reasm[c]
+        for r in recs[ok]:
+            su = r[:12].tobytes()
+            if self.emit_sus:
+                ev.append(self._event("su", c, t, su=su, index=int(r[13]), frame=int(r[14]) | (int(r[15]) << 8)))
+            rs.push_su(su)
+        for rec in rs.pop_all():
+            rec["record_kind"], rec["acars_mode"] = rec.pop("kind"), rec.pop("mode")
+            self._messages[c] += 1
+            ev.append(self._event("acars", c, t, **rec))
+        return ev
+
+    def _cframes(self, c, su, ok, voice, frame, t):
+        """carrier c's C-channel frames (read_frames arrays), decoded by input second t: counted -> their "cframe" events"""
+        ev = []
+        for k in range(len(frame)):
+            self._frames[c] += 1; self._su_total[c] += 3; self._su_bad[c] += int((ok[k] == 0).sum())
+            ev.append(self._event("cframe", c, t, sus=[x.tobytes() for x in su[k]], crc_ok=[bool(x) for x in ok[k]],
+                                  voice=voice[k].tobytes(), frame=int(frame[k])))
+        return ev
+
+
+class Receiver(_Events):
     """Decodes every continuous carrier of one wideband SDR IQ stream (cu8 or cs16 at any whole-hertz rate) on one GPU.
 
     Acquisition: the first acquire_seconds of IQ feed a Scanner (scan_nfft points) and are kept in one device buffer. Then
@@ -223,10 +260,6 @@ class Receiver:
         self._ticks += due
         return self._read()
 
-    def _event(self, kind, c, t, **fields):
-        car = self._carriers[c]
-        return dict(kind=kind, carrier=c, center_hz=car["center_hz"], mode=car["mode"], input_seconds=t, **fields)
-
     def _read(self):
         ev, t = [], self._n_in / self.input_rate
         for g in self._groups:
@@ -237,33 +270,6 @@ class Receiver:
             else:
                 for ch, (su, ok, voice, frame) in enumerate(g.layer.read_frames()):
                     ev += self._cframes(g.first + ch, su, ok, voice, frame, t)
-        return ev
-
-    def _units(self, c, recs, t):
-        """carrier c's signal-unit records (read_sus_raw rows), decoded by input second t: counted, the CRC-valid ones pushed to
-        the carrier's Reassembler -> their "su" (with emit_sus) and "acars" events"""
-        ev = []
-        ok = recs[:, 12] != 0
-        self._su_total[c] += len(recs); self._su_bad[c] += int((~ok).sum())
-        rs = self._reasm[c]
-        for r in recs[ok]:
-            su = r[:12].tobytes()
-            if self.emit_sus:
-                ev.append(self._event("su", c, t, su=su, index=int(r[13]), frame=int(r[14]) | (int(r[15]) << 8)))
-            rs.push_su(su)
-        for rec in rs.pop_all():
-            rec["record_kind"], rec["acars_mode"] = rec.pop("kind"), rec.pop("mode")
-            self._messages[c] += 1
-            ev.append(self._event("acars", c, t, **rec))
-        return ev
-
-    def _cframes(self, c, su, ok, voice, frame, t):
-        """carrier c's C-channel frames (read_frames arrays), decoded by input second t: counted -> their "cframe" events"""
-        ev = []
-        for k in range(len(frame)):
-            self._frames[c] += 1; self._su_total[c] += 3; self._su_bad[c] += int((ok[k] == 0).sum())
-            ev.append(self._event("cframe", c, t, sus=[x.tobytes() for x in su[k]], crc_ok=[bool(x) for x in ok[k]],
-                                  voice=voice[k].tobytes(), frame=int(frame[k])))
         return ev
 
     # ---------------------------------------------------------------------------------------------------------- state
