@@ -741,6 +741,13 @@ class RTChannelBatch(_Handle):
             res.append(pk)
         return res
 
+    def read_packets_raw(self, out, counts):
+        """The C-ABI call without per-channel Python objects, into out[n_channels, cap, RECORD] uint8 and counts[n_channels]
+        int32; record = int32 type (1 R, 2 T), nsus, payload bytes, start bit, then the payload. -> (out, counts)"""
+        assert out.dtype == np.uint8 and out.shape[0] == self.n and out.shape[2] == self.RECORD and out.flags.c_contiguous
+        _check(lib().jaero_rt_read_packets(self.h, _p(out), out.shape[1], _p(counts)))
+        return out, counts
+
     def stats(self):
         tr = np.zeros(self.n, dtype=np.int32); bad = np.zeros(self.n, dtype=np.int32); dcd = np.zeros(self.n, dtype=np.int32)
         _check(lib().jaero_rt_get_stats(self.h, _p(tr), _p(bad), _p(dcd)))
@@ -1215,3 +1222,4 @@ def probe_carriers(carriers, input_rate, iq, fmt, interpolation=1, decimation=No
 from .receiver import Receiver  # noqa: E402  (built on the classes above)
 from .recording import RecordingDecoder  # noqa: E402
 from .audio import AudioDecoder  # noqa: E402
+from .bursts import BurstAudioDecoder  # noqa: E402
